@@ -1,19 +1,25 @@
 #!/usr/bin/env python
 """bench.py -- BASELINE.json's metric: megapixels/s of fused BilateralSliceApply @4K.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step is ONE pass of the hot path over one batch of synthetic input: one launch of the fused
 slice-apply kernel over 8 frames of 3840x2160 (BASELINE.json configs[2]) per GPU, grid
-16x16x8x12, has_offset.  Inputs are device-resident before the timed region; 1.86 GB are
-touched per step, far more than the 126 MB L2, so no flush is needed between iterations.
-Multi-GPU: the batch shards over ranks with no data-path collective (weak scaling: 8 frames
-per GPU); timing is CUDA events on the launch stream, max over ranks.
+16x16x8x12, has_offset.  Inputs are device-resident before the timed region and drawn from
+fixed seeds, so they are identical from run to run; 1.86 GB are touched per step, far more
+than the 50 MB L2 of an H100, so no flush is needed between iterations.  Exactly K steps are
+timed.  Multi-GPU: the batch shards over ranks with no data-path collective (weak scaling: 8
+frames per GPU); timing is CUDA events on the launch stream, max over ranks.
 
-Rank 0 prints ONE JSON line (keys: see the task contract).  `--impl reference` times the
-reference's own CPU loops (oracle/_ref: hdrnet/ops/bilateral_slice_apply.cc compiled
-unmodified; falls back to the C restatement) on the host cores.
+Rank 0 prints ONE JSON line (the headline `value` and the records listed in run_b200_arm).
+`--impl reference` times the reference's own CPU loops (oracle/_ref: hdrnet/ops/
+bilateral_slice_apply.cc compiled unmodified; falls back to the C restatement) on the host cores.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed: a fixed,
+seeded sample of 4 Mi output pixels of rank 0 (DIR/slice_apply_out_sample.npy, float32
+[4194304, 3], 48 MB) -- so that two builds can be compared output for output.  Nothing else is
+written anywhere; the tree may be read-only.
 """
 from __future__ import annotations
 
@@ -59,17 +65,35 @@ def measured_peaks():
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
-def ncu_traffic_per_launch():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture, or None."""
-    path = os.path.join(ROOT, "profiles", "slice_apply_traffic.json")
+def gpu_identity(torch, index: int):
+    """Name, power limit and maximum SM clock of the card the numbers were measured on."""
+    import subprocess
+    rec = {"name": torch.cuda.get_device_name(index)}
     try:
-        with open(path) as f:
-            return json.load(f).get("dram_bytes_per_launch")
+        q = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit,clocks.max.sm",
+                            "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        if q.returncode == 0 and q.stdout.strip():
+            power, clock = (x.strip() for x in q.stdout.strip().splitlines()[0].split(","))
+            rec.update(power_limit=power, sm_max_clock=clock)
     except Exception:
-        return None
+        pass
+    return rec
+
+
+DUMP_SAMPLE_PX = 1 << 22   # 4 Mi pixels x 3 channels x 4 B = 48 MB
+
+
+def dump_outputs(torch, out, directory):
+    """A fixed, seeded sample of the output pixels (the same indices on every run of this shape)."""
+    os.makedirs(directory, exist_ok=True)
+    flat = out.reshape(-1, out.shape[-1])
+    gen = torch.Generator(device="cpu").manual_seed(2024)
+    idx = torch.randperm(flat.shape[0], generator=gen)[:DUMP_SAMPLE_PX].sort().values
+    sample = flat[idx.to(flat.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(directory, "slice_apply_out_sample.npy"), sample)
 
 
 class ClockSampler(threading.Thread):
@@ -135,13 +159,7 @@ def cpu_checker():
     # host threads it can, so undo that before libgomp is initialised by the oracle library.
     if os.environ.get("OMP_NUM_THREADS") in (None, "1"):
         os.environ["OMP_NUM_THREADS"] = str(os.cpu_count() or 1)
-    import oracle
-    if not oracle.have_ref() or not os.path.exists(os.path.join(ROOT, "oracle", "_build",
-                                                                "libhdrnet_oracle.so")):
-        try:
-            oracle.build()
-        except Exception:
-            pass
+    import oracle           # built by build(); nothing is compiled here
     return oracle.best()
 
 
@@ -349,7 +367,7 @@ def extra_records(torch, dist, lib, _lib, dev, stream, world, rank, peak, args):
             sweep[f"{gh}x{gw}x{gd}"] = _op_case(torch, lib, _lib, dev, stream, B_PER_GPU, H4K, W4K, gh, gw, gd, 30, peak)
         ex["C5_grid_sweep_4k_x8"] = sweep
         # the same shapes with a natural-image-like guide (the random one is the worst case for the
-        # shared-memory bank groups at 16 depth cells, DESIGN.md section 4)
+        # shared-memory bank groups at 16 depth cells)
         ex["C5_smooth_guide_4k_x8"] = {
             f"{gh}x{gw}x{gd}": _op_case(torch, lib, _lib, dev, stream, B_PER_GPU, H4K, W4K, gh, gw, gd, 30, peak,
                                         smooth_guide=True)
@@ -436,6 +454,8 @@ def run_b200_arm(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     elapsed_max_ms = float(t.item())
     own_launch_ms = elapsed_ms / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, out, args.dump_outputs)
 
     # ---- end to end: public API, pinned HOST buffers, H2D + kernel + D2H inside the timing --
     e2e_steps = max(1, min(args.steps, args.e2e_steps))
@@ -524,12 +544,13 @@ def run_b200_arm(args):
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "frames_per_gpu": B, "global_frames": B * world,
                        "parallelism": f"batch-shard x{world}, no data-path collective",
-                       "l2": "1.86 GB touched per step >> 126 MB L2: no flush between iterations",
+                       "l2": "1.86 GB touched per step >> 50 MB L2: no flush between iterations",
                        "kernel": {"variant": KERNEL_TEXT.get(variant.value, f"variant {variant.value}"),
                                   "ctas": ctas.value, "threads": threads.value,
                                   "dyn_smem_bytes": smem.value, "workspace_bytes": ws_bytes}},
+            "gpu": gpu_identity(torch, local_rank),
             "roofline": {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-                         "frac": round(achieved / peak, 4), "traffic": ncu_traffic_per_launch(),
+                         "frac": round(achieved / peak, 4),
                          "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": algo_bytes,
                          "launch_ms": round(own_launch_ms, 5),
@@ -574,7 +595,11 @@ def main():
     ap.add_argument("--e2e-steps", type=int, default=5)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra records (configs 2, 4, 5, model path)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed sample of the last timed step's output to DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
         return run_reference_arm(args)
     return run_b200_arm(args)

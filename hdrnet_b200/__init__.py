@@ -1,4 +1,4 @@
-"""hdrnet_b200 -- B200-native (sm_100a) implementation of google/hdrnet's bilateral-slice
+"""hdrnet_b200 -- H100-native (sm_90a) implementation of google/hdrnet's bilateral-slice
 hot path behind the reference's own ``hdrnet_ops`` / ``layers`` / ``models`` interface.
 
     from hdrnet_b200 import hdrnet_ops, layers, models

@@ -1,7 +1,7 @@
 """ctypes binding of libhdrnet_b200.so (the C-ABI declared in include/hdrnet_b200.h).
 
 The library is built in-tree (``hdrnet_b200/lib/``) by ``hdrnet_b200/csrc/Makefile`` for
-sm_100a.  There is NO fallback: if the library is missing or an op is called without a CUDA
+sm_90a.  There is NO fallback: if the library is missing or an op is called without a CUDA
 device, the call raises -- a silent CPU path would void every parity claim.
 """
 from __future__ import annotations
@@ -83,7 +83,7 @@ class HdrnetLibraryError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into hdrnet_b200/lib/ (nvcc cross-compiles
+    """Compile every CUDA source for sm_90a into hdrnet_b200/lib/ (nvcc cross-compiles
     without a GPU).  Returns the library path."""
     proc = subprocess.run(["make", "-C", CSRC_DIR, "-j8"], capture_output=True, text=True)
     if verbose or proc.returncode != 0:

@@ -10,8 +10,7 @@
 //                        conv (:129-132) and the unroll_grid permutation (:134-139) in one
 //                        pass, writing the [B,gh,gw,gd,n_out*n_in] grid slice-apply reads.
 //
-// The whole network is ~83 MFLOP per image: launch-latency bound, not tensor bound (DESIGN.md
-// section 5).  fp32 CUDA-core math keeps the coefficients within float32 round-off of the
+// The whole network is ~83 MFLOP per image: launch-latency bound, not tensor bound.  fp32 CUDA-core math keeps the coefficients within float32 round-off of the
 // float64-accumulated oracle, which bf16 / tf32 tensor-core math could not.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
@@ -38,7 +37,7 @@ struct ConvArgs {
 
 // Register tile per thread: kConvPx output pixels x kConvCo output channels.  <2, 8> is the
 // throughput shape (64 px x 32 channels per CTA); <1, 4> quadruples the CTA count for the
-// tiny late layers at batch 1, which are otherwise a handful of CTAs on 148 SMs.
+// tiny late layers at batch 1, which are otherwise a handful of CTAs on 132 SMs.
 template <int kConvPx, int kConvCo>
 __global__ void __launch_bounds__(kConvThreads)
 conv2d_nhwc_kernel(const ConvArgs a) {
@@ -123,7 +122,7 @@ conv2d_nhwc_kernel(const ConvArgs a) {
       if (vec_in && (cn % 4 == 0)) {
         // unrolled so that several iterations' input loads are in flight at once: a late layer at
         // batch 1 is a few dozen CTAs of 4 warps, and every new (tap, 4 channels) is an L2 round trip
-        // that nothing else on the SM hides (ncu: 31 us for 9.4 MMAC before; see tools/time_cnn.py)
+        // that nothing else on the SM hides (tools/time_cnn.py times the layers)
 #pragma unroll(kConvPx == 1 ? 8 : 4)
         for (int ci = 0; ci < cn; ci += 4) {
           float xin[kConvPx][4];
@@ -239,7 +238,7 @@ fc_kernel(const float* __restrict__ in, const float* __restrict__ w,
 
 // ---- fully connected, split-K over a thread-block cluster ----------------------------------------
 // At batch <= 8 a fully connected layer is a weight stream (fc1: 1 MB) that a handful of CTAs
-// cannot pull fast enough (52 us measured with 4 CTAs).  Here the K dimension is split over the
+// cannot pull fast enough.  Here the K dimension is split over the
 // CTAs of a cluster (up to 8): every CTA streams its slice of W with 128-bit loads (16 rows x 16
 // float4 columns in flight per pass), reduces its 16 row-lanes in shared memory, and the
 // cluster's rank 0 sums the per-CTA partials through DISTRIBUTED SHARED MEMORY in a fixed order
@@ -369,10 +368,10 @@ fuse_predict_kernel(const float* __restrict__ local, const float* __restrict__ g
   }
 }
 
-// conv_tcgen05.cu: tensor-core (tcgen05 / TMEM, 3xTF32) implicit-GEMM form of the same layer.
-int launch_conv_tcgen05(const float* in, const float* w, const float* bias, float* out, int B,
-                        int H, int W, int Cin, int Cout, int k, int stride, int relu, int OH,
-                        int OW, int pad_t, int pad_l, cudaStream_t stream);
+// conv_wgmma.cu: tensor-core (wgmma, 3xTF32) implicit-GEMM form of the same layer.
+int launch_conv_wgmma(const float* in, const float* w, const float* bias, float* out, int B,
+                      int H, int W, int Cin, int Cout, int k, int stride, int relu, int OH,
+                      int OW, int pad_t, int pad_l, cudaStream_t stream);
 
 static void same_pad(int size, int k, int s, int* out, int* before) {
   *out = (size + s - 1) / s;
@@ -384,7 +383,7 @@ static void same_pad(int size, int k, int s, int* out, int* before) {
 // ---------------------------------------------------------------------------------------------
 // Latency form for the small late layers (batch 1-2: a few thousand output pixels at most).
 // conv2d_nhwc_kernel walks its k*k*Cin reduction with one dependent L2 round trip per 4 input
-// channels and 4 warps per SM: ncu showed 17-29 us per layer for 2-9 MMAC (12 % issue-active).
+// channels and 4 warps per SM, mostly waiting on those round trips.
 // Here a CTA owns 32 output pixels (lane = pixel) x 4*kCoGroups output channels and
 //   1. copies every lane's k x k x Cin input patch and the CTA's weight columns into shared
 //      memory with 16-byte cp.async -- ALL of them in flight at once, one memory round trip;
@@ -829,7 +828,7 @@ static int conv_fill(ConvArgs* a, const float* in, const float* w, const float* 
 }
 
 static int device_sms() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;
@@ -852,25 +851,25 @@ static bool patch_two_groups(long long ctas1, int Cout, int K, int sms) {
 
 static int conv_dispatch(const ConvArgs& a, bool pdl, cudaStream_t stream) {
   if (a.B == 0) return HDRNET_OK;
-  {  // Tensor-core path (conv_tcgen05.cu).  Each 128-pixel tile runs a fixed-latency chunk loop,
-     // so it wins once there are about as many tiles as SMs (measured on B200: 2x faster at 128
-     // tiles, 3x slower at 2); HDRNET_CONV_TCGEN05=1 / =0 forces it on / off.
+  {  // Tensor-core path (conv_wgmma.cu).  Each 128-pixel tile runs a fixed-latency chunk loop,
+     // so it pays off once there are about as many tiles as SMs (H100, tools/conv_bench.py: about
+     // even with the CUDA-core kernels at 64 tiles, 1.8-3.7x faster at 128); HDRNET_CONV_TCGEN05=1
+     // / =0 forces it on / off.
     const char* e = std::getenv("HDRNET_CONV_TCGEN05");   // per call: tests and smoke() flip it in-process
     const long long tiles = (static_cast<long long>(a.B) * a.OH * a.OW + 127) / 128;
     const bool want = e ? (e[0] == '1') : (tiles >= 96);
     if (want) {
-      const int rc = launch_conv_tcgen05(a.in, a.w, a.bias, a.out, a.B, a.H, a.W, a.Cin, a.Cout, a.k, a.stride,
-                                         a.relu, a.OH, a.OW, a.pad_t, a.pad_l, stream);
+      const int rc = launch_conv_wgmma(a.in, a.w, a.bias, a.out, a.B, a.H, a.W, a.Cin, a.Cout, a.k, a.stride,
+                                       a.relu, a.OH, a.OW, a.pad_t, a.pad_l, stream);
       if (rc != HDRNET_E_UNSUPPORTED) return rc;
     }
   }
   const long long total_px = static_cast<long long>(a.B) * a.OH * a.OW;
   const int sms = device_sms();
   const long long big_ctas = ((total_px + 63) / 64) * ((a.Cout + 31) / 32);
-  // The shared-memory patch form: one memory round trip instead of one per 4 input channels.  It
-  // beats the register-tile kernels at every size measured (batch 1-8 of every layer of the
-  // network, tools/time_conv_layers.py: 2-3.5x at batch 1, 1.3-3x at batch 8); the bound below
-  // is where its 9x-redundant staging traffic was last measured, not a known crossover.
+  // The shared-memory patch form: one memory round trip instead of one per 4 input channels, for
+  // batch 1-8 of every layer of the network (tools/time_conv_layers.py compares the forms); the
+  // bound below caps its 9x-redundant staging traffic, it is not a measured crossover.
   if (patch_mode() != 0 && patch_ok(a)) {
     const long long tiles = (total_px + kPatchPx - 1) / kPatchPx;
     const long long ctas1 = tiles * (a.Cout / 4);

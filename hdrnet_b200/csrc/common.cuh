@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the bilateral-slice kernels (sm_100a).
+// common.cuh -- shared device helpers for the bilateral-slice kernels (sm_90a).
 //
 // Numerics contract (SURVEY.md section 7.3, BASELINE.json north_star):
 //   * cell-index arithmetic is BIT-EXACT with the reference:
@@ -91,8 +91,7 @@ __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v,
 
 // One 128-bit shared-memory load that the compiler may not split or rematerialise: under
 // register pressure nvcc turned `float4 g = guide4[tid]` into four LDS.32 issued right before
-// each use -- 4-way bank conflicted (lanes 16 B apart) -- which cost 6.6 % of the kernel's
-// shared-memory wavefronts (ncu source counters, profiles/).
+// each use -- 4-way bank conflicted (lanes 16 B apart).
 __device__ __forceinline__ float4 lds128(const void* p) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
@@ -101,7 +100,10 @@ __device__ __forceinline__ float4 lds128(const void* p) {
   return v;
 }
 
-// ---- packed fp32x2 math (Blackwell-only: fma.rn.f32x2 -> SASS FFMA2) --------------------
+// ---- fp32 pairs: two lanes of a 64-bit register pair, each rounded on its own ---------------
+// Hopper has no packed fp32 FMA, so a pair op is two scalar FFMA / FMUL.  Both halves use the
+// explicitly rounded intrinsics: nvcc may not contract a mul2 into a following fma2, which keeps
+// every blend bit-identical to the order written at the call site.
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
   unsigned long long r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -112,14 +114,17 @@ __device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& 
 }
 __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b,
                                                    unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
 // ---- programmatic dependent launch (sm_90+); both are no-ops in a grid launched without the

@@ -57,7 +57,7 @@ static int launch_guide(const float* rgb, float* guide, long long npix, const Fn
   if (npix == 0) return HDRNET_OK;
   if (!rgb || !guide) return HDRNET_E_NULL_POINTER;
   const bool vec_ok = ((reinterpret_cast<uintptr_t>(rgb) | reinterpret_cast<uintptr_t>(guide)) & 15u) == 0;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long work = vec_ok ? (npix + 3) / 4 : npix;

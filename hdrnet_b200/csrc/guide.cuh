@@ -43,7 +43,7 @@ struct NNGuideParams {
 
 __device__ __forceinline__ float curves_guide(const CurvesGuideParams& p, float r, float g,
                                               float b) {
-  // One FMNMX per knot and one packed FFMA2 per two knots (vs FADD + FMNMX + FFMA each).
+  // One FMNMX and one FFMA per knot (vs FADD + FMNMX + FFMA each).
   float acc = p.folded_bias;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -66,7 +66,7 @@ __device__ __forceinline__ float curves_guide(const CurvesGuideParams& p, float 
 // weight).  Weights beyond p.feats are zero (pack_nn_params), so the extra features add 0.
 template <int kFeats>
 __device__ __forceinline__ float nn_guide(const NNGuideParams& p, float r, float g, float b) {
-  // Two features per packed FFMA2; sigmoid through ex2.approx / rcp.approx: ~3e-7 absolute.
+  // Features in pairs (fma2); sigmoid through ex2.approx / rcp.approx: ~3e-7 absolute.
   const unsigned long long r2 = pack2(r, r), g2 = pack2(g, g), b2v = pack2(b, b);
   unsigned long long y2 = 0ull;
 #pragma unroll

@@ -47,7 +47,7 @@ extern "C" int hdrnet_resize_bilinear_f32(const float* in, const float* add, flo
   const float sy = (OH > 1) ? static_cast<float>(H - 1) / static_cast<float>(OH - 1) : 0.0f;
   const float sx = (OW > 1) ? static_cast<float>(W - 1) / static_cast<float>(OW - 1) : 0.0f;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   hdrnet_b200::resize_bilinear_ac_kernel<<<static_cast<unsigned>(blocks), 256, 0,
                                            static_cast<cudaStream_t>(stream)>>>(
       in, add, out, B, H, W, C, OH, OW, sy, sx, total);
@@ -102,7 +102,7 @@ extern "C" int hdrnet_lowres_nearest_f32(const void* image, int fmt, float* lowr
   if (total == 0) return HDRNET_OK;
   if (!image || !lowres) return HDRNET_E_NULL_POINTER;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const unsigned nb = static_cast<unsigned>(blocks);
   switch (fmt) {

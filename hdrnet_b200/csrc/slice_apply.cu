@@ -1,10 +1,11 @@
-// slice_apply.cu -- fused BilateralSliceApply for B200 (sm_100a), plus the generic
+// slice_apply.cu -- fused BilateralSliceApply for H100 (sm_90a), plus the generic
 // any-shape slice / slice-apply kernel and the cell-index debug kernel.
 //
 // Replaces hdrnet/ops/bilateral_slice_apply.cu.cc:36-126 (BilateralSliceApplyKernel, one
 // thread per OUTPUT ELEMENT, 32 scalar grid loads each, no shared memory) with a design
-// built around what bounds the op on B200: 28 B of HBM traffic per pixel against ~120-150
-// fp32 issue slots per pixel at the HBM roofline (DESIGN.md section 3).
+// built around what bounds the op: 28 B of HBM traffic per pixel against ~250 fp32 lane
+// operations per pixel at the HBM roofline (132 SMs x 128 lanes x ~1.8 GHz over 3.35 TB/s / 28 B;
+// DESIGN.md section 3).
 //
 // slice_apply_rows_tma_kernel -- persistent, one CTA per resident slot:
 //   * every HBM byte moves through the TMA engine: 1-D bulk copies (cp.async.bulk ->
@@ -15,7 +16,7 @@
 //   * the grid rows a pixel row touches (gy0, gy0+1: gw*gd*12 floats each) are staged once
 //     by TMA and stay resident while consecutive rows share them; per image row they are
 //     pre-blended along y (wy is constant on a row) into a slab Gy[gx][gz][12], so a pixel
-//     blends 4 corners instead of 8: 48 FMAs -> 24 packed fma.rn.f32x2 (FFMA2) + 9 for
+//     blends 4 corners instead of 8: 48 FMAs instead of 96, + 9 for
 //     the affine apply.
 //   * one thread owns 4 consecutive pixels: 3 LDS.128 of RGB + 1 LDS.128 of guide, 12
 //     16-byte slab chunks per pixel (conflict-free within an x cell: its 8 depth cells map to
@@ -31,8 +32,8 @@
 // guide sources, plan / argument structs), this file (generic kernels, the block-synchronous row
 // kernel, the un-fused slice kernel, the y pre-pass, planning, kernel selection, C-ABI),
 // slice_apply_async.cu (issuer-warp form: what AUTO runs for large images with a workspace).
-// Forms that measured slower (z-bucketed, texture-fed input, producer-warp, three tensor-core
-// gather forms) live in tools/experiments/ with their profiles; they are not part of the library.
+// Forms that measured slower (z-bucketed, texture-fed input, producer-warp, tensor-core gather
+// forms) are not part of the library.
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -133,7 +134,7 @@ slice_generic_kernel(const float* __restrict__ grid, const float* __restrict__ g
 // everything else -- has_offset = False (ops_test.py:345-365), other n_in / n_out
 // (HDRNetGaussianPyrNN's 9 x 4 grids sliced directly, hdrnet_ops_test.py:91-100), odd widths,
 // unaligned views, and the un-fused slice with gc != 12 -- used to fall to slice_generic_kernel:
-// 8 corners x gc scalar L2 loads per pixel, 16.7 % of the HBM roofline at 4K.
+// 8 corners x gc scalar L2 loads per pixel.
 // This kernel keeps what makes the row kernels fast and drops only the bulk copies: a persistent
 // CTA owns contiguous rows; the two grid rows a pixel row touches are staged in shared memory
 // (plain loads, reloaded only when the row pair changes) and pre-blended along y into a slab
@@ -518,7 +519,7 @@ slice_apply_rows_tma_kernel(const TmaArgs args, const __grid_constant__ GuideFn 
 // =========================================================================================
 // Same organisation as the fused kernel, but the op is WRITE-bound (4 B in, 48 B out per pixel):
 // the guide arrives through a deep ring of small TMA copies, each thread blends the 4 slab
-// corners of its pixels (24 FFMA2 per pixel, no apply) and writes the 12 coefficients into one of
+// corners of its pixels (48 FFMA per pixel, no apply) and writes the 12 coefficients into one of
 // kSliceOutBufs shared-memory output tiles that leave by TMA bulk stores; an mbarrier per
 // output tile (armed by the store-issuing thread after cp.async.bulk.wait_group.read) gates
 // its reuse.  Thread t owns pixels t and t + 256 of a 512-pixel segment: 48-byte stride between
@@ -712,11 +713,11 @@ static bool make_slice_plan(const SliceGeom& g, int max_smem, int sms, SlicePlan
 
 // Pre-pass of the texture-assisted forms: yslab[r] = (1 - fy) * G[b][gy0] + fy * G[b][gy1] for
 // every buffer row r = (b, y) -- the same y pre-blend the row kernel does in shared memory,
-// materialised once (gw*gd*48 B per image row: +11 % HBM traffic at 4K / 16x16x8).
+// materialised once (gw*gd*48 B per image row: +11 % HBM bytes at 4K / 16x16x8).
 // One CTA owns kYblendRows consecutive rows and a thread one output float4 column of them: the two
 // grid rows it blends change every H / gh image rows, so they live in registers and the kernel
-// is a stream of coalesced stores (the first version -- one CTA per row, two dependent L2 loads
-// per thread -- took 22 us for 106 MB, latency-bound).
+// is a stream of coalesced stores (one CTA per row, with two dependent L2 loads per thread, is
+// latency-bound).
 constexpr int kYblendRows = 16;
 __global__ void __launch_bounds__(256)
 yblend_rows_kernel(const float* __restrict__ grid, float4* __restrict__ ws, SliceGeom g,
@@ -758,9 +759,9 @@ static int launch_yblend(const float* grid, float* ws, const SliceGeom& g, int r
 
 static int device_sm_count() {
   int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 148;
-  return sms > 0 ? sms : 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
+  return sms > 0 ? sms : 132;
 }
 
 static int device_max_smem_optin() {
@@ -866,8 +867,8 @@ static int launch_tma(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream, 
     if (a.p.threads == 512) return launch_tma_occ<GuideFn, kTexChunks, 2, 512>(a, fn, stream);
   } else {
     // The fused-guide forms are issue-bound and need their registers: 256 threads x 2 CTAs.
-    // Measured at 4K x 8 (tools/ab_fused.py): curves 0.69 ms against 0.71 (256 x 3) and 0.80
-    // (512 x 2); pointwise NN 0.63 / 0.69 / 0.72.  Integer pixel formats exist for them only.
+    // (chosen against 256 x 3 and 512 x 2 on the previous target; not re-tuned on H100).  Integer
+    // pixel formats exist for them only.
     if (in_fmt == kPxU8 && out_fmt == kPxU8)
       return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU8, kPxU8>(a, fn, stream);
     if (in_fmt == kPxU16 && out_fmt == kPxU8)
@@ -1059,10 +1060,8 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
                                        kPxF32, kPxF32, 2, /*grid_rows=*/2) &&
                          splan.resident == 2 && splan.seg_px <= splan.threads * 4 && splan.stages >= kAsyncAutoMinStages;
   if (slab_warp) aplan = splan;
-  // ... and its fused-guide forms (8 math warps + the issuer).  Measured at 4K x 8
-  // (profiles/r02_ab_fused_issuer_warp.txt): curves 0.628 ms against 0.700 block-synchronous (u8:
-  // 0.668 / 0.729); pointwise NN 0.628 / 0.625 (u8: 0.694 / 0.654) -- AUTO takes it for the
-  // curves guide only.
+  // ... and its fused-guide forms (8 math warps + the issuer).  AUTO takes it for the curves guide
+  // only: for the pointwise-NN guide the block-synchronous form was as fast.
   TmaPlan fplan;
   const bool fused_async_ok = tex_ok && gs.mode != 0 &&
                               make_tma_plan(g, max_smem, sms, &fplan, /*tex_mode=*/true, kFusedAsyncMathThreads,

@@ -14,8 +14,8 @@ namespace hdrnet_b200 {
 // =========================================================================================
 // Issuer-warp form of the texture-assisted row kernel (HDRNET_VARIANT_TEX_ASYNC).
 // =========================================================================================
-// What the block-synchronous kernel loses (ncu, profiles/r01_final_ncu_full_summary.txt): 1.8
-// barrier stalls per issue and ~116 warp instructions per item outside the pixel body.  After
+// What the block-synchronous kernel loses: barrier stalls, and warp instructions per item spent
+// outside the pixel body.  After
 // every segment's __syncthreads thread 0 runs a SERIAL section (bulk store, wait for the previous
 // store, an integer division for the next item, expect_tx, two bulk loads) while its own warp's
 // pixels wait -- so warp 0 reaches the next barrier late by that section and the other fifteen
@@ -40,9 +40,9 @@ namespace hdrnet_b200 {
 // instead of FRND + F2I (two).  t_i, the fractions and every weight are computed by the same
 // rounded operations as spatial_axis / range_axis: results are bitwise those of the other forms.
 //
-// Tried on this form and removed (results in DESIGN.md section 3): results stored by STG.128 from
-// registers (+10 %), slab rows blended by the issuer warp from L2 (2x slower), texture fetches
-// software-pipelined one pixel ahead (no gain), programmatic dependent launch of the pre-pass (+14 %).
+// Tried on this form and removed because they were slower or no faster: results stored by STG.128
+// from registers, slab rows blended by the issuer warp from L2, texture fetches software-pipelined
+// one pixel ahead, programmatic dependent launch of the pre-pass.
 
 // Which of a pixel's 12 corner chunks -- corner c = 0..3 (v00, v01, v10, v11), part p = 0..2 --
 // travel through the texture pipe: the last kTexChunks of the ids 3 c + p.
@@ -216,7 +216,7 @@ __device__ __forceinline__ void process_quad_lean_fused(const TmaArgs& args, con
 // warps -- from the two grid rows it keeps staged in shared memory (TMA, reloaded only when the pair
 // changes) into (i) the shared-memory slab buffer the LSU chunks are read from and (ii) the row's
 // place in the caller's workspace, from where the texture chunks are fetched a row later.  The
-// separate pre-pass launch (21 us, 5 % of the step at 8 x 4K) and the slab-row bulk loads
+// separate pre-pass launch and the slab-row bulk loads
 // disappear.  A CTA only ever fetches workspace rows its own slab warp wrote earlier in this launch
 // (a row split between two CTAs is written by both, with identical bytes), after a device-scope
 // fence and the slab barrier; L1 / texture caches start a launch invalid, so no stale line of an
@@ -239,8 +239,8 @@ slice_apply_rows_async_kernel(const TmaArgs args) {
   unsigned char* raw0 = smem + pl.off_raw;               // two slab rows
   unsigned char* stage_base = smem + pl.off_stage;
 
-  // Work split in ITEMS (row segments), not rows: 17280 rows over 296 CTAs leave some CTAs 59 rows
-  // and others 58 (1.1 % of the kernel is the tail); in half-row items the imbalance is 0.2 %.
+  // Work split in ITEMS (row segments), not rows: 17280 rows (4K x 8) over 264 CTAs give 120 CTAs
+  // 66 rows and 144 CTAs 65, a tail of one whole row; in half-row items the tail is half a row.
   // A CTA covers items [i_begin, i_end): rows r_begin .. r_end-1, the first row from pixel
   // x_first, the last row up to pixel x_last (a row split between two CTAs has its slab row
   // loaded by both).

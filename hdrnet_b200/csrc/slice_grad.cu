@@ -269,7 +269,7 @@ static int launch_grads(const float* grid, const float* guide, const float* inpu
                         cudaStream_t stream) {
   const long long npix = static_cast<long long>(g.B) * g.H * g.W;
   if (npix == 0) return HDRNET_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int gc = g.n_out * g.J;

@@ -103,13 +103,15 @@ __device__ __forceinline__ float load_channel(const unsigned char* base, long lo
 
 constexpr int kTmaThreads = 256;
 constexpr int kTmaThreadsDefault = 256;  // all-LSU form
-constexpr int kTexThreadsDefault = 512;  // block-synchronous texture-assisted form: measured 7 % faster at 512 (64 registers)
+constexpr int kTexThreadsDefault = 512;  // block-synchronous texture-assisted form (64 registers)
 constexpr int kFusedThreadsDefault = 256; // fused-guide forms of the block-synchronous kernel
 constexpr int kAsyncThreadsDefault = 352; // issuer-warp form: 10 math warps + the issuer, two CTAs per SM, 88 registers
-                                          // (same-box A/B, profiles/r02_ab_async_pipe.txt: 0.4451 ms against 0.4563 at 512)
 // AUTO takes the issuer-warp form only with a ring of >= 3 stages at two CTAs per SM: with the two
-// stages that 32x32 grids leave (24 / 48 KB of slab rows) it measured SLOWER than the
-// block-synchronous form (32x32x8: 46.9 % vs 53.2 % of HBM peak; 32x32x16: 31.1 % vs 37.5 %).
+// stages that 32x32 grids leave (24 / 48 KB of slab rows) the block-synchronous form was faster.
+// Checked on an H100 (tools/ab_lib.py, 4K x 8, medians of interleaved bursts, 400 W card): at
+// 16x16x8 the default (352 + slab warp, 5 texture chunks) 0.805 ms against 0.827 without the slab
+// warp, 0.838 with 4 texture chunks, 0.841 at 512 threads, 0.931 block-synchronous texture form,
+// 0.949 all-LSU; at 32x32x16 1.258 against 1.255 (4 chunks), 1.388 (512), 1.370 (block-synchronous).
 constexpr int kAsyncAutoMinStages = 3;
 constexpr int kAsyncTexChunksDefault = 5; // corner chunks per pixel through the texture pipe (HDRNET_TEX_CHUNKS)
 constexpr int kAsyncSlabWarpDefault = 1;  // slab rows blended by a slab warp inside the kernel: no pre-pass (HDRNET_ASYNC_SLAB)
@@ -291,8 +293,8 @@ __device__ __forceinline__ void process_quad(const TmaArgs& args, const GuideFn&
 int launch_async_form(const TmaArgs& a, int chunks, bool lean, int threads, bool slab_warp, cudaStream_t stream);
 int launch_async_fused(const TmaArgs& a, int mode, const CurvesGuideParams* curves, const NNGuideParams* nn,
                        int in_fmt, int out_fmt, cudaStream_t stream);
-// fused-guide issuer-warp form: 8 math warps + the issuer warp, 2 CTAs per SM (96 registers).  Measured
-// against 6 math warps x 3 CTAs and 10 x 2 (both 80 registers) at 4K x 8, curves guide: 0.608 / 0.687 / 0.670 ms.
+// fused-guide issuer-warp form: 8 math warps + the issuer warp, 2 CTAs per SM (96 registers); preferred
+// to 6 math warps x 3 CTAs and 10 x 2 (both 80 registers) for the curves guide.
 constexpr int kFusedAsyncMathThreads = 256;
 constexpr int kFusedAsyncResident = 2;
 

@@ -3,7 +3,7 @@
 The reference binds ``bilateral_slice`` / ``bilateral_slice_apply`` from a TF op library
 (hdrnet/hdrnet_ops.py:23-31).  Here the same two names take ``torch.Tensor`` arguments in the
 same order, with the same shapes (TF NHWC) and the same ``has_offset`` attribute, and call
-the hand-written sm_100a kernels through the C-ABI (include/hdrnet_b200.h):
+the hand-written sm_90a kernels through the C-ABI (include/hdrnet_b200.h):
 
     bilateral_slice(grid[B,gh,gw,gd,gc], guide[B,H,W])                      -> [B,H,W,gc]
     bilateral_slice_apply(grid, guide, input[B,H,W,n_in], has_offset)        -> [B,H,W,n_out]
@@ -36,7 +36,7 @@ _host_ctx = {}  # device index -> hdrnet_host_ctx*
 def _require_cuda() -> None:
     if not torch.cuda.is_available():
         raise _lib.HdrnetLibraryError(
-            "hdrnet_b200 needs a CUDA device (sm_100a); there is no CPU implementation")
+            "hdrnet_b200 needs a CUDA device (sm_90a); there is no CPU implementation")
 
 
 def _f32c(t: torch.Tensor, what: str) -> torch.Tensor:

@@ -6,8 +6,8 @@ runs, the prediction comes back.  ``models.*.inference_image`` is that per-frame
 image already on the device; this module is the part around it for a batch / stream of frames
 that lives in (pinned) host memory: three CUDA streams -- copy-in, compute, copy-out -- so that
 frame i + 1 is uploading and frame i - 1 is downloading while frame i computes.  For 4K uint8
-frames the model takes ~0.25 ms of GPU time per frame against ~0.5 ms per direction over PCIe, so
-a pipelined batch approaches the PCIe time of ONE direction instead of the sum of
+frames the model's GPU time per frame is well below a frame's PCIe time in one direction, so a
+pipelined batch approaches the PCIe time of ONE direction instead of the sum of
 upload + compute + download.
 
 Device buffers are owned by the pipeline (``depth`` frames in, the model's outputs are held until

@@ -16,7 +16,7 @@ flat dict of numpy arrays keyed by the SAME variable names under ``inference/``
 install it once with ``set_weights`` / ``load_weights``.  Conv weights are HWIO, FC weights
 [in, out], exactly as TF stores them.
 
-Execution (all hand-written sm_100a kernels through the C-ABI, no torch math on the path):
+Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
   coefficients  4 splat convs, 2 global convs + 3 FCs, 2 local convs (conv2d / fc kernels),
                 then fusion + prediction + unroll_grid in one kernel -> grid [B,gh,gw,gd,12]
   guide+output  ONE kernel: per-pixel guide (curves or pointwise NN) computed in registers
@@ -149,8 +149,7 @@ def init_weights(params, seed: int = 0, model_name: str | None = None) -> dict:
 # (hdrnet_coefficients_f32, csrc/cnn.cu: 8 launches chained with programmatic dependent launch, the
 # global and local branches sharing launches, fc1-fc3 in one cluster) instead of twelve per-layer
 # calls from Python; larger batches go layer by layer so that the convs can use the packed
-# tensor-core weights.  Measured (tools/time_cnn.py): the chain wins up to batch 16 (221 vs 234 us),
-# loses at 64 (596 vs 487 us).  Tests set this to force either path.
+# tensor-core weights (tools/time_cnn.py times both).  Tests set this to force either path.
 CHAIN_CNN_MAX_BATCH = 16
 
 _host_pipelines = {}   # (model class, device, out dtype) -> HostImagePipeline (inference_image_host)
@@ -299,7 +298,7 @@ def quantize_u8(x: torch.Tensor) -> torch.Tensor:
 
 
 def pack_conv_weights(w: torch.Tensor):
-    """Pre-pack HWIO conv weights for the pipelined tcgen05 kernel (once per model); returns a
+    """Pre-pack HWIO conv weights for the pipelined tensor-core (wgmma) kernel (once per model); returns a
     device buffer, or None when the layer's shape does not suit that kernel."""
     lib = _lib.load()
     k, _, cin, cout = w.shape
@@ -316,14 +315,14 @@ def pack_conv_weights(w: torch.Tensor):
 
 def _use_packed_tc(tiles: int) -> bool:
     """HDRNET_CONV_TCGEN05: '1' = tensor-core convs wherever weights were packed, '0' = never.
-    Default: from 8 tiles of 128 output pixels up -- the measured crossover on B200
-    (profiles/r01_conv_tcgen05_vs_cudacore.txt: slower than the CUDA-core kernel at 2 tiles,
-    faster from batch 8, 5x faster at batch 64)."""
+    Default: from 64 tiles of 128 output pixels up.  Measured on an H100 (tools/conv_bench.py, the
+    network's conv shapes): at 16 tiles the CUDA-core kernels were 3-15 % faster, at 64 the two
+    were even, at 128 the packed tensor-core kernel was 1.7-5x faster."""
     import os
     flag = os.environ.get("HDRNET_CONV_TCGEN05")
     if flag is not None:
         return flag == "1"
-    return tiles >= 8
+    return tiles >= 64
 
 
 def _conv(x: torch.Tensor, wb, stride=1, relu=True) -> torch.Tensor:
@@ -342,7 +341,7 @@ def _conv(x: torch.Tensor, wb, stride=1, relu=True) -> torch.Tensor:
                                            W, cin, cout, k, stride, int(relu),
                                            torch.cuda.current_stream(x.device).cuda_stream)
         if rc != _lib.E_UNSUPPORTED:
-            _lib.check(rc, "conv2d(tcgen05)")
+            _lib.check(rc, "conv2d(tensor cores)")
             return out
     rc = lib.hdrnet_conv2d_nhwc_f32(x.data_ptr(), w.data_ptr(), 0 if b is None else b.data_ptr(),
                                     out.data_ptr(), B, H, W, cin, cout, k, stride, int(relu),

@@ -5,7 +5,7 @@ grid / guide / input (hdrnet/ops/bilateral_slice_apply.cu.cc:67-125 -- the batch
 selects slabs), and the coefficient network is per-image (hdrnet/models.py:63, :95).  So the
 design is one process per GPU, images sharded over ranks, and exactly ONE collective: a
 broadcast of the flat coefficient-network weight buffer (~1.93 MB) at init over NCCL
-(NVLink 5 / NVSwitch); "nccl" on GPUs, "gloo" in the CPU tests.  The reference itself has no
+(NVLink / NVSwitch); "nccl" on GPUs, "gloo" in the CPU tests.  The reference itself has no
 distributed code at all (SURVEY.md section 2b).
 """
 from __future__ import annotations
@@ -44,8 +44,7 @@ def bind_to_gpu_numa(device_index: int) -> list[int]:
     """Pin this process (and the threads it starts later: the host path's copy threads, pinned
     allocations' first touch) to the CPUs local to its GPU.  Call BEFORE allocating pinned host
     memory: with eight ranks feeding 1.9 GB per step each, buffers that land on the other socket
-    cross the inter-socket link on every H2D / D2H copy (SCALE_r01: end-to-end efficiency 0.45 at
-    8 GPUs with device-timed 0.99).  Returns the CPU list it bound to ([] = left unbound)."""
+    cross the inter-socket link on every H2D / D2H copy.  Returns the CPU list it bound to ([] = left unbound)."""
     cpus = gpu_cpu_affinity(device_index)
     if not cpus:
         return []

@@ -1,5 +1,5 @@
 /*
- * hdrnet_b200.h -- C-ABI of libhdrnet_b200.so: the B200 (sm_100a) implementation of
+ * hdrnet_b200.h -- C-ABI of libhdrnet_b200.so: the H100 (sm_90a) implementation of
  * google/hdrnet's bilateral-slice hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / TF types.  Each entry
@@ -67,7 +67,7 @@ extern "C" {
                                  /* instead of block barriers) + one warp that issues every  */
                                  /* bulk copy; per-quad index arithmetic.  Same requirements */
                                  /* as HDRNET_VARIANT_TEX.  (Values 3, 5, 6, 8-11 named forms */
-                                 /* that measured slower; they live in tools/experiments/.)   */
+                                 /* that measured slower; they are not part of the library.) */
 HDRNET_API int hdrnet_b200_abi_version(void);
 
 /* Human-readable text for a return code of this library (static storage). */
@@ -236,8 +236,8 @@ HDRNET_API int hdrnet_conv2d_nhwc_f32(const float* in, const float* w, const flo
                                       int stride, int relu, void* stream);
 
 /*
- * Tensor-core form of conv2d (tcgen05.mma kind::tf32 with 3xTF32 operand splitting, accumulator
- * in TMEM; float32-grade results).  Weights are packed ONCE per model into per-chunk hi/lo tiles
+ * Tensor-core form of conv2d (wgmma.mma_async .tf32 with 3xTF32 operand splitting, fp32
+ * accumulator; float32-grade results).  Weights are packed ONCE per model into per-chunk hi/lo tiles
  * in the MMA's shared-memory layout (hdrnet_conv2d_tc_packed_bytes() bytes, device memory owned
  * by the caller); the layer call then needs Cin % 4 == 0, Cout % 16 == 0, 16 <= Cout <= 128.
  * hdrnet_conv2d_nhwc_f32 also reaches an unpacked tensor-core kernel on its own when the layer
@@ -272,7 +272,7 @@ HDRNET_API int hdrnet_fuse_predict_f32(const float* local, const float* global_f
  * and the local branch (both read the splat features) share a launch per depth, fc1-fc3 run in one
  * 8-CTA cluster with activations in distributed shared memory -- chained with programmatic
  * dependent launch so that each layer's launch and weight fetch overlap the previous layer's tail
- * (batch 1: 65 us against 150 us for twelve per-layer calls, tools/time_cnn.py).
+ * (tools/time_cnn.py compares it with twelve per-layer calls).
  *   lowres [B, S, S, 3] float32 -> grid [B, sb, sb, gd, n_out, n_in] float32
  *   weights / biases: HOST arrays of n_layers = n_ds + 8 DEVICE pointers (n_ds = log2(S / sb)), in
  *     the order splat conv1..n_ds, global conv1, conv2, fc1, fc2, fc3, local conv1, conv2,

@@ -12,10 +12,11 @@ cross-checked against each other and against the reference's known-answer tests 
 ``port``      ``hdrnet_oracle.c`` -- plain-C float32 restatement of
               hdrnet/ops/bilateral_slice{,_apply}.cc + numerics.h, OpenMP over rows.
 ``ref``       the reference's own .cc files compiled unmodified into ``oracle/_ref/``
-              (``oracle/Makefile``; needs /root/reference at build time only).
+              (``oracle/Makefile``; needs a google/hdrnet checkout -- HDRNET_REFERENCE, default
+              /root/reference -- at build time only; the .so then travels with the tree).
 ``jax_shim``  the reference's own jax/bilateral_slice.py imported under a numpy stand-in
-              for jax (works only where /root/reference is mounted; it generated the
-              fixtures in tests/golden/).
+              for jax (works only where that checkout is readable; it generated the fixtures in
+              tests/golden/).
 ``model_np``  numpy restatement of hdrnet/models.py + layers.py (coefficient CNN, guides).
 """
 from __future__ import annotations
@@ -35,7 +36,7 @@ _i32p = ctypes.POINTER(ctypes.c_int32)
 
 
 def build(verbose: bool = False) -> None:
-    """Compile the C restatement and, when /root/reference is mounted, ``oracle/_ref``."""
+    """Compile the C restatement and, where the reference checkout is readable, ``oracle/_ref``."""
     out = subprocess.run(["make", "-C", _HERE, "all"], capture_output=True, text=True)
     if verbose or out.returncode != 0:
         print(out.stdout, out.stderr)

@@ -1,11 +1,13 @@
 """Run the reference's own ``jax/bilateral_slice.py`` without JAX -- TEST INFRASTRUCTURE ONLY.
 
-The parity target BASELINE.json names is ``/root/reference/jax/bilateral_slice.py``
-(``bilateral_slice`` :299-380, numerics in ``jax/numerics.py``).  JAX is not installed in
-this image, so this module injects a small numpy stand-in for ``jax`` / ``jax.numpy`` into
+The parity target BASELINE.json names is the reference's ``jax/bilateral_slice.py``
+(``bilateral_slice`` :299-380, numerics in ``jax/numerics.py``), found in the google/hdrnet
+checkout that the environment variable ``HDRNET_REFERENCE`` points to (default: ``DEFAULT_REFERENCE``,
+where the build environment mounts it).  JAX need not be
+installed: this module injects a small numpy stand-in for ``jax`` / ``jax.numpy`` into
 ``sys.modules`` and then imports the two reference files UNMODIFIED from where they lie.
-Nothing is copied; if ``/root/reference`` is absent (the GPU box) ``load()`` raises and the
-callers use the committed fixtures in ``tests/golden/`` instead.
+Nothing is copied; without a checkout ``load()`` raises, and the tests use the fixtures that
+``tests/golden/make_golden.py`` stored from it.
 
 Stand-in semantics that matter for parity:
 * ``jnp.arange`` returns int32 (as JAX does with x64 disabled);
@@ -25,7 +27,8 @@ import types
 
 import numpy as np
 
-REFERENCE_JAX_DIR = "/root/reference/jax"
+DEFAULT_REFERENCE = "/root/reference"   # same default as oracle/Makefile
+REFERENCE_JAX_DIR = os.path.join(os.environ.get("HDRNET_REFERENCE") or DEFAULT_REFERENCE, "jax")
 
 
 class _F32Int(np.ndarray):
@@ -130,7 +133,7 @@ _loaded = None
 
 
 def available() -> bool:
-    return os.path.exists(os.path.join(REFERENCE_JAX_DIR, "bilateral_slice.py"))
+    return os.access(os.path.join(REFERENCE_JAX_DIR, "bilateral_slice.py"), os.R_OK)
 
 
 def load():
@@ -139,7 +142,8 @@ def load():
     if _loaded is not None:
         return _loaded
     if not available():
-        raise FileNotFoundError(f"{REFERENCE_JAX_DIR} not mounted; use tests/golden fixtures")
+        raise FileNotFoundError(f"no readable google/hdrnet checkout at {os.path.dirname(REFERENCE_JAX_DIR)} "
+                                "(HDRNET_REFERENCE); the tests use tests/golden fixtures")
     saved = {k: sys.modules.get(k) for k in ("jax", "jax.numpy")}
     jnp = _make_jnp()
     jax = _make_jax(jnp)

@@ -1,7 +1,7 @@
 // ref_capi.cc -- C entry points around the REFERENCE's own CPU loops.
 //
 // TEST INFRASTRUCTURE ONLY (oracle/).  oracle/Makefile compiles this file together with
-// /root/reference/hdrnet/ops/bilateral_slice.cc and bilateral_slice_apply.cc -- taken where
+// the reference checkout's hdrnet/ops/bilateral_slice.cc and bilateral_slice_apply.cc -- taken where
 // they lie, UNMODIFIED, never copied into this repo -- against oracle/nda_standin (a
 // stand-in for the un-vendored nda header) into oracle/_ref/libhdrnet_ref.so.
 //

@@ -1,6 +1,7 @@
 """Generate the golden fixtures in tests/golden/ from the REFERENCE itself.
 
-Run in the build container (needs /root/reference):   python tests/golden/make_golden.py
+Needs a google/hdrnet checkout and its compiled loops (oracle/_ref, built by oracle.build()):
+    HDRNET_REFERENCE=<checkout> python tests/golden/make_golden.py [vjp | live]
 
 Outputs are produced by the reference's own jax/bilateral_slice.py (:299-380), imported
 unmodified under the numpy stand-in for jax (oracle/jax_shim.py), and -- for slice-apply --
@@ -16,8 +17,13 @@ reference's tests:
   vjp_*              the reference's own VJPs of the slice (jax/bilateral_slice.py:26-108, :257-295) at
                      the extents of its gradient tests (hdrnet_ops_test.py:91-100, :185-195) and on a
                      grid coarser / finer than the image; `python make_golden.py vjp` writes only these
+  live_reference     what tests/test_oracle.py compares the port with when the reference is at hand:
+                     the JAX file's outputs on a signed case, its grid VJP at an exact cell centre,
+                     and SHA-256 digests of the compiled C++ loops' outputs (the port must be
+                     bit-exact, so a digest is the whole comparison); `python make_golden.py live`
 Each .npz stores inputs, outputs and the reference's cell indices.
 """
+import hashlib
 import os
 import sys
 
@@ -25,6 +31,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.normpath(os.path.join(HERE, "..", "..")))
+sys.path.insert(0, os.path.normpath(os.path.join(HERE, "..")))
 
 from oracle import jax_shim  # noqa: E402
 
@@ -87,10 +94,11 @@ def main():
     inp = rng.rand(1, 7, 4, 3).astype(np.float32)
     save("edge_gd1", **case(grid, guide, inp))
 
-    # Wide enough for the TMA row kernel (W % 4 == 0, W >= 128), ragged last segment.
+    # Wide enough for the TMA row kernel (W % 4 == 0, W >= 128), ragged last segment; 4 rows keep
+    # the fixture under 1 MB.
     grid = rng.rand(2, 4, 6, 8, 12).astype(np.float32)
-    guide = rng.rand(2, 6, 1100).astype(np.float32)
-    inp = rng.rand(2, 6, 1100, 3).astype(np.float32)
+    guide = rng.rand(2, 4, 1100).astype(np.float32)
+    inp = rng.rand(2, 4, 1100, 3).astype(np.float32)
     save("wide_rows", **case(grid, guide, inp))
 
 
@@ -110,7 +118,47 @@ def main_vjp():
         save(f"vjp_{k}", grid=grid, guide=guide, codomain_tangent=ct, grid_vjp=gv, guide_vjp=uv)
 
 
+def sha256(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def main_live():
+    """Inputs are regenerated by the tests from tests/util.py rand_case; only outputs are stored."""
+    import oracle
+    from util import rand_case
+    grid, guide, inp = rand_case(11, 2, 40, 36, 8, 6, 5, signed=True)
+    d = dict(jax_slice=jax_shim.bilateral_slice(grid, guide),
+             jax_apply_offset=jax_shim.bilateral_slice_apply(grid, guide, inp, True),
+             jax_indices=jax_shim.slice_indices(guide, 8, 6, 5))
+    # grid VJP where guide * gd - 0.5 is an exact integer (tests/test_oracle.py, cell-centre test)
+    gh, gw, gd, gc, h, w = 3, 2, 4, 1, 6, 5
+    rng = np.random.RandomState(11)
+    g = rng.rand(1, h, w).astype(np.float32)
+    g[0, 2, 3] = 1.5 / gd
+    ct = rng.randn(1, h, w, gc).astype(np.float32)
+    d["jax_cell_centre_grid_vjp"], _ = jax_shim.bilateral_slice_vjp(np.zeros((1, gh, gw, gd, gc), np.float32), g, ct)
+    ref = oracle.ref()
+    for k, shape in enumerate([(3, 30, 25, 16, 12, 8), (2, 64, 48, 3, 5, 4), (1, 8, 5, 6, 3, 7)]):
+        grid, guide, inp = rand_case(99, *shape, signed=True)
+        digests = [sha256(ref.bilateral_slice_apply(grid, guide, inp, ho))
+                   for ho in (True, False) if grid.shape[-1] % (3 + ho) == 0]
+        digests.append(sha256(ref.bilateral_slice(grid, guide)))
+        d[f"ref_forward_sha256_{k}"] = np.array(digests)
+    B, H, W, gh, gw, gd, n_in, n_out = 3, 8, 5, 6, 3, 7, 3, 4
+    grid, guide, inp = rand_case(5, B, H, W, gh, gw, gd, n_in, n_out, True)
+    rng = np.random.RandomState(6)
+    ct = rng.rand(B, H, W, n_out).astype(np.float32)
+    digests = [sha256(a) for a in ref.bilateral_slice_apply_grad(grid, guide, inp, ct, True)]
+    ct = rng.rand(B, H, W, grid.shape[-1]).astype(np.float32)
+    digests += [sha256(a) for a in ref.bilateral_slice_grad(grid, guide, ct)]
+    d["ref_vjp_sha256"] = np.array(digests)
+    save("live_reference", **d)
+
+
 if __name__ == "__main__":
-    if sys.argv[1:] != ["vjp"]:
-        main()
-    main_vjp()
+    if sys.argv[1:] == ["live"]:
+        main_live()
+    else:
+        if sys.argv[1:] != ["vjp"]:
+            main()
+        main_vjp()

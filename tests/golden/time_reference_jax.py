@@ -1,10 +1,10 @@
 """Times the reference's own JAX file (jax/bilateral_slice.py:299-380, imported unmodified under the
 numpy stand-in, oracle/jax_shim.py) + the reference's `apply` (hdrnet/layers.py:153-198) on THIS
-machine's host cores: BASELINE.md section 3's "R-JAX" row.  It needs /root/reference, which exists in
-the build container only (the GPU box has none: bench.py's CPU legs time the reference's compiled C++
-loops there instead), so this is a reported-only number recorded by hand in profiles/.
+machine's host cores: BASELINE.md section 3's "R-JAX" row.  It needs a google/hdrnet checkout
+(HDRNET_REFERENCE); bench.py's CPU legs time the reference's compiled C++ loops (or the C
+restatement) instead, so this is a reported-only number.
 
-    python tests/golden/time_reference_jax.py [H W]        # default: one 1080 x 1920 frame
+    HDRNET_REFERENCE=<checkout> python tests/golden/time_reference_jax.py [H W]   # default: one 1080 x 1920 frame
 """
 import os
 import platform

@@ -44,9 +44,9 @@ def test_ctypes_table_covers_the_header(built_lib):
     assert "NULL" in _lib.error_string(_lib.E_NULL_POINTER)
 
 
-def test_library_is_built_for_sm_100a(built_lib):
+def test_library_is_built_for_sm_90a(built_lib):
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True)
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout
 
 
 def test_product_never_imports_the_oracle():
@@ -169,23 +169,23 @@ def _plan(lib, B, H, W, gh, gw, gd, with_ws, n_in=3, n_out=3, has_offset=1):
 
 
 def test_kernel_selection_plan(built_lib):
-    """Host-side kernel selection (no launch; without a device the planner assumes a B200: 148 SMs,
+    """Host-side kernel selection (no launch; without a device the planner assumes an H100: 132 SMs,
     227 KB of opt-in shared memory): which form AUTO runs for BASELINE.json's shapes."""
     from hdrnet_b200 import _lib
     lib = built_lib
-    # config 3 (headline): issuer-warp texture-assisted form, 2 CTAs x 148 SMs, 10 math warps + issuer
+    # config 3 (headline): issuer-warp texture-assisted form, 2 CTAs x 132 SMs, 10 math warps + issuer
     # + slab warp (no pre-pass), 4-stage ring of 1280-pixel segments + 2 slab rows + 2 grid rows
-    assert _plan(lib, 8, 2160, 3840, 16, 16, 8, 1) == (_lib.VARIANT_TEX_ASYNC, 296, 384, 106752)
+    assert _plan(lib, 8, 2160, 3840, 16, 16, 8, 1) == (_lib.VARIANT_TEX_ASYNC, 264, 384, 106752)
     # no workspace lent: the all-LSU TMA row kernel
     v, c, t, _ = _plan(lib, 8, 2160, 3840, 16, 16, 8, 0)
-    assert (v, c, t) == (_lib.VARIANT_TMA, 296, 256)
+    assert (v, c, t) == (_lib.VARIANT_TMA, 264, 256)
     # config 4 (12 MP, 8 frames per GPU): three 1344-pixel segments per row, 4-stage ring
     v, c, t, sm = _plan(lib, 8, 3024, 4032, 16, 16, 8, 1)
-    assert (v, c, t) == (_lib.VARIANT_TEX_ASYNC, 296, 384) and sm <= 115712
+    assert (v, c, t) == (_lib.VARIANT_TEX_ASYNC, 264, 384) and sm <= 115712
     # config 5's 32x32 grids (24 / 48 KB of slab rows) still leave the 20 KB stages a 3-stage ring;
     # 32x32x16 has no room for two more grid rows: pre-pass form (352 threads)
-    assert _plan(lib, 8, 2160, 3840, 32, 32, 8, 1)[:3] == (_lib.VARIANT_TEX_ASYNC, 296, 384)
-    assert _plan(lib, 8, 2160, 3840, 32, 32, 16, 1)[:3] == (_lib.VARIANT_TEX_ASYNC, 296, 352)
+    assert _plan(lib, 8, 2160, 3840, 32, 32, 8, 1)[:3] == (_lib.VARIANT_TEX_ASYNC, 264, 384)
+    assert _plan(lib, 8, 2160, 3840, 32, 32, 16, 1)[:3] == (_lib.VARIANT_TEX_ASYNC, 264, 352)
     assert _plan(lib, 8, 2160, 3840, 8, 8, 4, 1)[0] == _lib.VARIANT_TEX_ASYNC
     # config 2 (one 1080p frame, < 2 Mi px): no pre-pass, TMA row kernel
     assert _plan(lib, 1, 1080, 1920, 16, 16, 8, 1)[0] == _lib.VARIANT_TMA

@@ -338,7 +338,7 @@ def test_run_py_identity_sample_plumbing(tmp_path):
     assert np.abs(out8.astype(int) - ref8.astype(int)).max() <= 1
 
 
-# ---- tcgen05 (tensor-core, 3xTF32) form of the conv layers ------------------------------------
+# ---- tensor-core (wgmma, 3xTF32) form of the conv layers (named after the HDRNET_CONV_TCGEN05 knob) ----
 @pytest.fixture
 def tcgen05_convs(monkeypatch):
     monkeypatch.setenv("HDRNET_CONV_TCGEN05", "1")
@@ -353,9 +353,11 @@ def tcgen05_convs(monkeypatch):
     (2, 32, 32, 32, 64, 3, 2, True, True),     # splat conv4, stride 2, SAME pad 0/1
     (3, 16, 16, 64, 96, 1, 1, False, True),    # 1x1 prediction, N = 96
     (1, 9, 7, 8, 16, 3, 1, True, True),        # ragged tile (63 px), K = 72 (partial last chunk)
+    (1, 16, 16, 64, 192, 3, 1, True, True),    # Cout > 128: two launches over columns 0-127, 128-191
+    (2, 12, 12, 32, 144, 3, 2, False, True),   # Cout = 128 + 16, stride 2
 ])
 def test_conv2d_tcgen05_matches_oracle(tcgen05_convs, B, H, W, cin, cout, k, stride, relu, bias):
-    """3xTF32 on tcgen05 keeps float32-grade accuracy: 1e-5 of the tensor's range (a plain
+    """3xTF32 on the tensor cores keeps float32-grade accuracy: 1e-5 of the tensor's range (a plain
     TF32 product would be ~1e-3)."""
     rng = np.random.RandomState(11)
     x = rng.randn(B, H, W, cin).astype(np.float32)
@@ -384,7 +386,7 @@ def test_coefficients_with_tcgen05_convs(tcgen05_convs):
     low = np.random.RandomState(4).rand(2, 256, 256, 3).astype(np.float32)
     ref = M.coefficients(low, wts, p)
     got = models.HDRNetCurves._coefficients(cuda(low), dict(p, weights=wts)).cpu().numpy()
-    assert_parity(got, ref, rtol=5e-5, what="coefficients via tcgen05 convs")
+    assert_parity(got, ref, rtol=5e-5, what="coefficients via tensor-core convs")
 
 
 # ---- HDRNetGaussianPyrNN (row f-2) -------------------------------------------------------------

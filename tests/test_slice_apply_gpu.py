@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA kernels, called through the C-ABI, against
+"""GPU parity tests (run on an H100): the CUDA kernels, called through the C-ABI, against
 the oracle on the same seeded inputs, against the committed golden fixtures from the
 reference's JAX file, and -- at BASELINE.json's full 4K size -- against the full oracle on
 one frame plus size-independent properties.  Tolerance: 1e-5 relative (tests/util.py);

@@ -78,9 +78,9 @@ lines = []
 for spec, v in res.items():
     t = [x[0] for x in v]
     med = statistics.median(t)
-    lines.append(f"{spec:70s} median {med:.4f} ms  min {min(t):.4f}  max {max(t):.4f}  frac {B*H*W*28/med/1e6/6577.4:.4f}")
+    lines.append(f"{spec:70s} median {med:.4f} ms  min {min(t):.4f}  max {max(t):.4f}  frac {B*H*W*28/med/1e6/3350.0:.4f}")
     lines.append("    bursts " + " ".join(f"{x[0]:.4f}@{x[1]}" for x in v))
 lines.append(f"all outputs bitwise equal: {equal}")
 print("\n".join(lines))
-os.makedirs("gpurun_out", exist_ok=True)
-open("gpurun_out/ab_lib.txt", "w").write("# tools/ab_lib.py " + " ".join(sys.argv[1:]) + "\n" + "\n".join(lines) + "\n")
+os.makedirs("tools_out", exist_ok=True)
+open("tools_out/ab_lib.txt", "w").write("# tools/ab_lib.py " + " ".join(sys.argv[1:]) + "\n" + "\n".join(lines) + "\n")

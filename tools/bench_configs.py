@@ -14,7 +14,7 @@ ROOT = os.path.normpath(os.path.join(os.path.dirname(os.path.abspath(__file__)),
 sys.path.insert(0, ROOT)
 from hdrnet_b200 import _lib, hdrnet_ops, models  # noqa: E402
 
-PEAK = 6577.4
+PEAK = 3350.0   # H100 SXM data sheet, GB/s
 try:
     PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:

@@ -1,11 +1,11 @@
 // cabi_check.cu -- torch-free check of a slice-apply kernel variant through the C-ABI: a few
-// seconds on a GPU box instead of a Python start-up (meant for the first runs of an untested
-// variant; the experimental forms of tools/experiments/ were brought up with it).
+// seconds on a GPU machine instead of a Python start-up (meant for the first runs of an untested
+// variant).
 //   nvcc -O2 -std=c++17 -I include -o tools/ubench/bin/cabi_check tools/cabi_check.cu -ldl
 //   tools/ubench/bin/cabi_check [variant=8] [B=2] [H=64] [W=3840] [gh=16] [gw=16] [gd=8] [iters=20]
 // Compares `variant` with HDRNET_VARIANT_GENERIC (one thread per pixel, the reference's own
 // summation order) on seeded random inputs -- max |diff| / max |ref|, bar 1e-5 -- runs it twice
-// (barrier phases / TMEM of a second launch), then times `iters` launches with CUDA events.
+// (barrier phases of a second launch), then times `iters` launches with CUDA events.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 

@@ -19,10 +19,10 @@ for B in (1, 8, 64):
         packed = models.pack_conv_weights(w)
         res.append(t(lambda: models._conv(x, (w, b, packed), stride=s)))
         flops = 2 * B * (H // s) ** 2 * cout * k * k * cin
-        print(f"B={B} {H}x{H}x{cin}->{cout} k{k}s{s}: cuda-core {res[0]:.1f} us, tcgen05 {res[1]:.1f} us, tcgen05 pipelined+packed {res[2]:.1f} us ({flops/res[2]/1e6:.2f} TFLOP/s eff.)")
+        print(f"B={B} {H}x{H}x{cin}->{cout} k{k}s{s}: cuda-core {res[0]:.1f} us, tensor cores {res[1]:.1f} us, tensor cores pipelined+packed {res[2]:.1f} us ({flops/res[2]/1e6:.2f} TFLOP/s eff.)")
 p = dict(models.DEFAULT_PARAMS); p["weights"] = models.init_weights(p, 0)
 for B in (1, 8):
     low = torch.rand(B, 256, 256, 3, device="cuda")
     for flag in ("0", "1"):
         os.environ["HDRNET_CONV_TCGEN05"] = flag
-        print("coefficient CNN B=%d tcgen05=%s: %.1f us" % (B, flag, t(lambda: models.HDRNetCurves._coefficients(low, p))))
+        print("coefficient CNN B=%d tensor-core convs=%s: %.1f us" % (B, flag, t(lambda: models.HDRNetCurves._coefficients(low, p))))

@@ -1,6 +1,6 @@
 """One markdown row per distinct kernel of an `ncu --page raw --csv` export (longest launch of each):
 duration, DRAM bytes and GB/s against the measured HBM peak, tensor-pipe / LSU-wavefront / issue
-utilisation, registers.    python tools/ncu_kernel_table.py raw.csv > profiles/<name>.md"""
+utilisation, registers.    python tools/ncu_kernel_table.py raw.csv > <name>.md"""
 import csv, json, os, re, sys
 
 rows = list(csv.reader(open(sys.argv[1])))
@@ -9,7 +9,7 @@ col = {k: i for i, k in enumerate(hdr)}
 try:
     peak = float(json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:
-    peak = 6650.0
+    peak = 3350.0
 
 
 def num(row, key, default=0.0):

@@ -1,8 +1,8 @@
 """Runs every kernel of libhdrnet_b200.so once at a representative shape, for one ncu pass:
-    ncu --set full --clock-control none -k regex:'hdrnet_b200' -c 200 -f -o gpurun_out/r02_all_kernels \
+    ncu --set full --clock-control none -k regex:'hdrnet_b200' -c 200 -f -o tools_out/r02_all_kernels \
         python tools/prof_all_kernels.py
-    ncu -i gpurun_out/r02_all_kernels.ncu-rep --page raw --csv > gpurun_out/r02_all_kernels_raw.csv
-    python tools/ncu_kernel_table.py gpurun_out/r02_all_kernels_raw.csv > profiles/r02_all_kernels_ncu.md
+    ncu -i tools_out/r02_all_kernels.ncu-rep --page raw --csv > tools_out/r02_all_kernels_raw.csv
+    python tools/ncu_kernel_table.py tools_out/r02_all_kernels_raw.csv > tools_out/all_kernels_ncu.md
 Synthetic inputs, seeded synthetic weights.  No warm-up on purpose (every launch is captured)."""
 import os, sys
 import numpy as np
@@ -20,7 +20,7 @@ def params(name, **kw):
     return p
 
 
-# ---- model path at 4K x 8: batch-8 CNN (tcgen05 packed convs, fc, fuse_predict), fused-guide slice-apply
+# ---- model path at 4K x 8: batch-8 CNN (tensor-core packed convs, fc, fuse_predict), fused-guide slice-apply
 im = torch.rand(8, 2160, 3840, 3, device=dev, generator=gen)
 for name in ("HDRNetCurves", "HDRNetPointwiseNNGuide"):
     p = params(name, batch_norm=(name != "HDRNetCurves"))

@@ -2,7 +2,7 @@
 import os, sys, json, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from hdrnet_b200 import hdrnet_ops
-PEAK = json.load(open("MEASURED_PEAKS.json")).get("hbm_gbs", 6577.4) if os.path.exists("MEASURED_PEAKS.json") else 6577.4
+PEAK = json.load(open("MEASURED_PEAKS.json")).get("hbm_gbs", 3350.0) if os.path.exists("MEASURED_PEAKS.json") else 3350.0
 
 def t(fn, iters=20):
     for _ in range(3): fn()

@@ -5,7 +5,7 @@ Run once per setting of HDRNET_CONV_PATCH (read once per process):
     HDRNET_CONV_PATCH=1 python tools/time_conv_layers.py   # patch form, 4 channels per CTA
     HDRNET_CONV_PATCH=2 python tools/time_conv_layers.py   # patch form, 8 channels per CTA
 Also prints max |diff| against the tensor-core-free HDRNET_CONV_PATCH=0 result when
-gpurun_out/conv_ref.pt exists (written by the =0 run).
+tools_out/conv_ref.pt exists (written by the =0 run).
 """
 import os, sys, statistics, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -18,7 +18,7 @@ LAYERS = [  # name, H, Cin, Cout, stride
 ]
 mode = os.environ.get("HDRNET_CONV_PATCH", "auto")
 lib = _lib.load()
-ref_path = "gpurun_out/conv_ref.pt"
+ref_path = "tools_out/conv_ref.pt"
 ref = torch.load(ref_path) if (mode != "0" and os.path.exists(ref_path)) else {}
 save = {}
 for B in (1, 2, 8):
@@ -51,5 +51,5 @@ for B in (1, 2, 8):
         line.append(f"{name} {statistics.median(ts):.1f}{d}")
     print(f"PATCH={mode} batch {B}: " + "  ".join(line), flush=True)
 if mode == "0":
-    os.makedirs("gpurun_out", exist_ok=True)
+    os.makedirs("tools_out", exist_ok=True)
     torch.save(save, ref_path)

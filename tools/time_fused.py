@@ -4,7 +4,7 @@ the CURRENT environment (HDRNET_FUSED_ASYNC = unset / 0 / 1 is read once per pro
 import os, sys, statistics, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from hdrnet_b200 import models, _lib
-if os.environ.get("HDRNET_LIB_OVERRIDE"):      # an experimental build (tools/experiments/lib_alt*)
+if os.environ.get("HDRNET_LIB_OVERRIDE"):      # another build of the library, for an A/B
     _lib.LIB_PATH = os.path.abspath(os.environ["HDRNET_LIB_OVERRIDE"])
 if os.environ.get("HDRNET_FUSED_ASYNC") == "":
     del os.environ["HDRNET_FUSED_ASYNC"]

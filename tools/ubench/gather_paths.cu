@@ -1,7 +1,7 @@
 // gather_paths.cu -- microbenchmark: which on-chip paths can carry a data-dependent 4-byte /
 // 16-byte table lookup per lane, and do they add up?  (Design input for the slice kernel's
 // corner gather, which ncu shows bound by shared-memory wavefronts.)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench/bin/gather_paths tools/ubench/gather_paths.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench/bin/gather_paths tools/ubench/gather_paths.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -96,8 +96,8 @@ int main() {
   float4* gtab; int* zs; float* out; long long* cyc;
   CK(cudaMalloc(&gtab, 8 * 3 * 16 * sizeof(float4)));
   CK(cudaMalloc(&zs, 4096 * sizeof(int)));
-  CK(cudaMalloc(&out, 148 * 8 * THREADS * sizeof(float) * 2));
-  CK(cudaMalloc(&cyc, 148 * 8 * sizeof(long long) * 2));
+  CK(cudaMalloc(&out, 132 * 8 * THREADS * sizeof(float) * 2));
+  CK(cudaMalloc(&cyc, 132 * 8 * sizeof(long long) * 2));
   std::vector<float4> h(8 * 3 * 16); for (size_t i = 0; i < h.size(); ++i) h[i] = make_float4(i, i + 1, i + 2, i + 3);
   std::vector<int> hz(4096); srand(1); for (auto& v : hz) v = rand() & 7;
   CK(cudaMemcpy(gtab, h.data(), h.size() * sizeof(float4), cudaMemcpyHostToDevice));

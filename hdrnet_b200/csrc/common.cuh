@@ -212,4 +212,44 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// ---- L2 eviction priorities (cache-policy operands of the .L2::cache_hint forms) -------------
+// evict_first: data touched once (streamed pixels) goes first, so it does not push out lines that
+// will be read again soon; evict_last: data written now and read back later in the same launch.
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// tma_load_1d / tma_store_1d with an L2 cache policy.
+__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes,
+                                            uint64_t* bar, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1], %2, [%3], %4;"
+      ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_1d(void* gmem_dst, const void* smem_src, uint32_t bytes,
+                                             uint64_t policy) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
+               ::"l"(gmem_dst), "r"(smem_u32(smem_src)), "r"(bytes), "l"(policy)
+               : "memory");
+}
+// One 16-byte global store with an L2 cache policy.
+__device__ __forceinline__ void st_global_hint(float4* p, const float4& v, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
+               ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(policy)
+               : "memory");
+}
+// Drop the 128-byte L2 line at p (128-byte aligned) without writing it back: the line's memory
+// holds undefined bytes afterwards.  For scratch data no one reads again.
+__device__ __forceinline__ void l2_discard_line(const void* p) {
+  asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory");
+}
+
 }  // namespace hdrnet_b200

@@ -275,6 +275,16 @@ slice_apply_rows_async_kernel(const TmaArgs args) {
     uint32_t gpar0 = 0u, gpar1 = 0u;
     const int n4 = pl.row_floats / 4;
     float4* ws4 = reinterpret_cast<float4*>(const_cast<float*>(args.yslab));
+    const uint64_t ws_pol = l2_policy_evict_last();
+    // Once the issuer has released a row every texture fetch of it has returned: a row this CTA
+    // owns whole (no other CTA fetches it) is dropped from L2 without a write-back to HBM.  Rows
+    // are whole 128-byte lines (slab_lines in launch_slice_apply_impl); the workspace's contents
+    // are undefined after the call.
+    auto discard_row = [&](long long r) {
+      if (row_x0(r) != 0 || row_x1(r) != g.W) return;
+      const unsigned char* base = reinterpret_cast<const unsigned char*>(ws4 + static_cast<size_t>(r) * n4);
+      for (int l = lane; l < static_cast<int>(slab_bytes / 128u); l += 32) l2_discard_line(base + 128 * l);
+    };
     for (long long row = r_begin; row < r_end; ++row) {
       const int rowk = static_cast<int>(row - r_begin), rb = rowk & 1;
       const int b = static_cast<int>(row / g.rows);
@@ -306,19 +316,27 @@ slice_apply_rows_async_kernel(const TmaArgs args) {
       for (int e = lane; e < n4; e += 32) {   // exactly yblend_rows_kernel's arithmetic
         const float4 v = lerp4(wy0, a4[e], wy1, b4[e]);
         slab4[e] = v;
-        wrow[e] = v;
+        st_global_hint(wrow + e, v, ws_pol);   // kept in L2 until the texture chunks have read it
       }
       __threadfence();   // the workspace row is visible device-wide before anyone is told it exists
       __syncwarp();
       if (lane == 0) arrive(&slab_full[rb]);
+      if (rowk >= 2) discard_row(row - 2);   // released: waited on row_free above
+    }
+    for (long long row = max(r_begin, r_end - 2); row < r_end; ++row) {   // the last two rows
+      const int rowk = static_cast<int>(row - r_begin);
+      mbar_wait(&row_free[rowk & 1], static_cast<uint32_t>(rowk >> 1) & 1u);
+      discard_row(row);
     }
     return;
   }
 
   if (warp == kMathWarps) {
     // ------------------------------- issuer warp --------------------------------------------
-    // Lane 0 issues every bulk copy.
+    // Lane 0 issues every bulk copy.  Pixels are touched once: evict_first keeps them from pushing
+    // the slab rows out of L2 between their write and their texture fetches.
     if (lane != 0) return;
+    const uint64_t px_pol = l2_policy_evict_first();
     auto make_slab = [&](long long row) {   // the row's y-pre-blended slab, from the pre-pass workspace
       if constexpr (kSlabWarp) return;
       const int rb = static_cast<int>(row - r_begin) & 1;
@@ -335,8 +353,8 @@ slice_apply_rows_async_kernel(const TmaArgs args) {
       unsigned char* st = stage_base + static_cast<size_t>(l_s) * pl.stage_bytes;
       const size_t pix = static_cast<size_t>(l_row) * g.W + l_x0;
       mbar_expect_tx(&full[l_s], static_cast<uint32_t>(npx) * 16u);
-      tma_load_1d(st, args.input + pix * 12, static_cast<uint32_t>(npx) * 12u, &full[l_s]);
-      tma_load_1d(st + pl.off_guide, args.guide + pix, static_cast<uint32_t>(npx) * 4u, &full[l_s]);
+      tma_load_1d(st, args.input + pix * 12, static_cast<uint32_t>(npx) * 12u, &full[l_s], px_pol);
+      tma_load_1d(st + pl.off_guide, args.guide + pix, static_cast<uint32_t>(npx) * 4u, &full[l_s], px_pol);
       if (++l_s == NS) l_s = 0;
       l_x0 += pl.seg_px;
       if (l_x0 >= row_x1(l_row)) { l_x0 = 0; ++l_row; }
@@ -355,7 +373,7 @@ slice_apply_rows_async_kernel(const TmaArgs args) {
         const int npx = min(pl.seg_px, g.W - x0);
         unsigned char* st = stage_base + static_cast<size_t>(s) * pl.stage_bytes;
         const size_t pix = static_cast<size_t>(row) * g.W + x0;
-        tma_store_1d(args.out + pix * 12, st, static_cast<uint32_t>(npx) * 12u);
+        tma_store_1d(args.out + pix * 12, st, static_cast<uint32_t>(npx) * 12u, px_pol);
         tma_store_commit();
         if (l_row < r_end) {
           tma_store_wait_read<1>();  // the previous item's store has drained the stage refilled now

@@ -94,6 +94,9 @@ HDRNET_API int hdrnet_slice_apply_f32_variant(const float* grid, const float* gu
  * Same op with a caller-provided device workspace (the library itself never allocates):
  * required by HDRNET_VARIANT_TEX, ignored by the other variants.
  * hdrnet_slice_apply_workspace_bytes() = B * H * gw * gd * 48.
+ * The workspace is scratch: its contents are undefined after a call (the kernels may drop rows
+ * they are done with from L2 without writing them back), and a call never reads what an earlier
+ * call left there.
  */
 HDRNET_API size_t hdrnet_slice_apply_workspace_bytes(int B, int H, int gw, int gd);
 HDRNET_API int hdrnet_slice_apply_f32_ws(const float* grid, const float* guide,

@@ -8,7 +8,7 @@ import torch
 
 import oracle
 from hdrnet_b200 import hdrnet_ops
-from util import assert_parity, rand_case
+from util import APPLY_CASES, SLICE_CASES, assert_parity, rand_case
 
 pytestmark = pytest.mark.gpu
 
@@ -17,15 +17,6 @@ def cuda(a, grad=False):
     t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
     return t.requires_grad_(grad)
 
-
-# (B, H, W, gh, gw, gd, n_in, n_out, has_offset)
-APPLY_CASES = [
-    (3, 8, 5, 6, 3, 7, 3, 4, True),      # hdrnet_ops_test.py:185-195 (generic grid-VJP path: gc=16)
-    (3, 30, 25, 16, 12, 8, 3, 3, True),  # default test extents: fast column kernel (gd<=8, gc<=12)
-    (2, 40, 64, 4, 4, 8, 3, 3, True),    # several pixels per cell, mirror boundary on all sides
-    (2, 33, 47, 5, 3, 4, 3, 4, False),   # no offset
-    (1, 16, 16, 2, 2, 1, 1, 1, True),    # gd = 1: both depth borders at once
-]
 
 
 @pytest.mark.parametrize("case", APPLY_CASES, ids=str)
@@ -49,8 +40,7 @@ def test_slice_apply_vjps_match_reference(case):
         assert_parity(got.cpu().numpy(), ref, rtol=2e-5, what=f"{case} {name} VJP")
 
 
-@pytest.mark.parametrize("case", [(3, 30, 25, 16, 12, 8, 12), (2, 21, 36, 5, 4, 6, 2), (1, 9, 7, 3, 3, 9, 5)],
-                         ids=str)
+@pytest.mark.parametrize("case", SLICE_CASES, ids=str)
 def test_slice_vjps_match_reference(case):
     B, H, W, gh, gw, gd, gc = case
     rng = np.random.RandomState(7)
@@ -167,3 +157,120 @@ def test_sgd_convergence_bounds_of_the_reference_tests(name):
     with torch.no_grad():
         final = float((target - forward()).square().sum())
     assert final < c["bound"], f"{name}: final loss {final:.3e} >= {c['bound']:.1e}"
+
+
+# ---- the autograd boundary ------------------------------------------------------------------
+def _apply_grads(grid, guide, inp, ct, wants=(True, True, True)):
+    g, u, i = cuda(grid, wants[0]), cuda(guide, wants[1]), cuda(inp, wants[2])
+    hdrnet_ops.bilateral_slice_apply(g, u, i, True).backward(ct if torch.is_tensor(ct) else cuda(ct))
+    torch.cuda.synchronize()
+    return [None if t.grad is None else t.grad.clone() for t in (g, u, i)]
+
+
+def _boundary_case(seed=3, B=2, H=40, W=56):
+    grid, guide, inp = rand_case(seed, B, H, W, 5, 7, 8, 3, 3, True, signed=True)
+    ct = np.random.RandomState(seed + 1).randn(B, H, W, 3).astype(np.float32)
+    return grid, guide, inp, ct
+
+
+def _equal(a, b):
+    return all((x is None and y is None) or torch.equal(x, y) for x, y in zip(a, b))
+
+
+def test_non_contiguous_upstream_gradients():
+    """A channel-reordered or transposed output hands backward a non-contiguous gradient; it must
+    give what its contiguous copy gives, bitwise."""
+    grid, guide, inp, ct = _boundary_case()
+    want = _apply_grads(grid, guide, inp, ct)
+    # the gradient arrives as a transposed view of a contiguous [B, W, H, C] tensor
+    ct_t = cuda(ct).transpose(1, 2).contiguous().transpose(1, 2)
+    assert not ct_t.is_contiguous()
+    assert _equal(_apply_grads(grid, guide, inp, ct_t), want)
+    # through an index and a transpose in the graph
+    g, u, i = cuda(grid, True), cuda(guide, True), cuda(inp, True)
+    out = hdrnet_ops.bilateral_slice_apply(g, u, i, True)
+    (out[..., [2, 1, 0]].transpose(1, 2) * cuda(ct[..., [2, 1, 0]]).transpose(1, 2)).sum().backward()
+    torch.cuda.synchronize()
+    assert _equal([g.grad, u.grad, i.grad], want)
+
+
+def test_only_some_inputs_require_grad():
+    grid, guide, inp, ct = _boundary_case()
+    want = _apply_grads(grid, guide, inp, ct)
+    for wants in ((False, True, False), (True, False, False), (False, False, True)):
+        got = _apply_grads(grid, guide, inp, ct, wants)
+        assert _equal(got, [w if f else None for w, f in zip(want, wants)]), wants
+    # bilateral_slice with only the guide, then only the grid
+    sct = np.random.RandomState(9).randn(*guide.shape, grid.shape[-1]).astype(np.float32)
+    ref = oracle.port().bilateral_slice_grad(grid, guide, sct)
+    for k in (0, 1):
+        g, u = cuda(grid, k == 0), cuda(guide, k == 1)
+        hdrnet_ops.bilateral_slice(g, u).backward(cuda(sct))
+        assert (g.grad is None) == (k == 1) and (u.grad is None) == (k == 0)
+        assert_parity((g.grad if k == 0 else u.grad).cpu().numpy(), ref[k], rtol=2e-5,
+                      what=f"slice VJP {k}", elem_rtol=None)
+
+
+def test_gradients_accumulate_over_two_backward_calls():
+    grid, guide, inp, ct = _boundary_case()
+    want = _apply_grads(grid, guide, inp, ct)
+    g, u, i = cuda(grid, True), cuda(guide, True), cuda(inp, True)
+    for _ in range(2):
+        hdrnet_ops.bilateral_slice_apply(g, u, i, True).backward(cuda(ct))
+    torch.cuda.synchronize()
+    assert _equal([g.grad, u.grad, i.grad], [2 * w for w in want])
+
+
+def test_backward_on_a_side_stream():
+    """The VJPs launch on the current stream: forward and backward on a side stream, queued behind
+    other work there, give the default stream's gradients, bitwise."""
+    grid, guide, inp, ct = _boundary_case()
+    want = _apply_grads(grid, guide, inp, ct)
+    s = torch.cuda.Stream()
+    busy = torch.randn(4096, 4096, device="cuda")
+    g, u, i = cuda(grid, True), cuda(guide, True), cuda(inp, True)
+    c = cuda(ct)
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(3):
+            busy = busy @ busy.T / 4096.0
+        hdrnet_ops.bilateral_slice_apply(g, u, i, True).backward(c)
+    torch.cuda.synchronize()
+    assert _equal([g.grad, u.grad, i.grad], want)
+
+
+def test_six_d_grids_through_layers():
+    """layers.bilateral_slice_apply takes [B,gh,gw,gd,n_out,n_in+1] (output-major) and
+    layers.bilateral_slice [B,gh,gw,gd,n_out,n_in] (packed input-major): their gradients are the
+    5-D op's, moved back through the same packing."""
+    from hdrnet_b200 import layers
+    grid, guide, inp, ct = _boundary_case()
+    B, gh, gw, gd, gc = grid.shape
+    want = _apply_grads(grid, guide, inp, ct)
+    g6 = cuda(grid.reshape(B, gh, gw, gd, 3, 4), True)
+    u, i = cuda(guide, True), cuda(inp, True)
+    layers.bilateral_slice_apply(g6, u, i, True).backward(cuda(ct))
+    torch.cuda.synchronize()
+    assert _equal([g6.grad.reshape(grid.shape), u.grad, i.grad], want)
+
+    # slice: 6-D channel (i, j) is 5-D channel j * n_out + i
+    grid6 = np.ascontiguousarray(grid.reshape(B, gh, gw, gd, 4, 3).transpose(0, 1, 2, 3, 5, 4))  # n_out=3, n_in=4
+    sct6 = np.random.RandomState(5).randn(*guide.shape, 3, 4).astype(np.float32)
+    grid5 = grid6.transpose(0, 1, 2, 3, 5, 4).reshape(B, gh, gw, gd, 12)
+    sct5 = sct6.transpose(0, 1, 2, 4, 3).reshape(*guide.shape, 12)
+    g5, u5 = cuda(grid5, True), cuda(guide, True)
+    hdrnet_ops.bilateral_slice(g5, u5).backward(cuda(sct5))
+    g6, u6 = cuda(grid6, True), cuda(guide, True)
+    layers.bilateral_slice(g6, u6).backward(cuda(sct6))
+    torch.cuda.synchronize()
+    back = g5.grad.reshape(B, gh, gw, gd, 4, 3).permute(0, 1, 2, 3, 5, 4)
+    assert torch.equal(g6.grad, back) and torch.equal(u6.grad, u5.grad)
+
+
+def test_permuting_the_batch_permutes_every_gradient():
+    grid, guide, inp, ct = _boundary_case(B=4)
+    perm = np.array([2, 0, 3, 1])
+    want = _apply_grads(grid, guide, inp, ct)
+    got = _apply_grads(grid[perm], guide[perm], inp[perm], ct[perm])
+    idx = torch.from_numpy(perm).cuda()
+    assert _equal(got, [w[idx] for w in want])

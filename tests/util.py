@@ -54,6 +54,21 @@ def assert_parity(actual, expected, rtol=RTOL, what="", elem_rtol=ELEM_RTOL):
                                        f"{per_elem:.3e} > {elem_rtol:.1e} (global {err:.3e})")
 
 
+# VJP test extents shared by tests/test_grad_gpu.py (CUDA vs the reference loops) and
+# tests/test_slice_f64.py (the float64 reference vs the same loops).
+# (B, H, W, gh, gw, gd, n_in, n_out, has_offset)
+APPLY_CASES = [
+    (3, 8, 5, 6, 3, 7, 3, 4, True),      # hdrnet_ops_test.py:185-195 (gc=16: two channel tiles)
+    (3, 30, 25, 16, 12, 8, 3, 3, True),  # default test extents: one column tile (gd<=8, gc<=12)
+    (2, 40, 64, 4, 4, 8, 3, 3, True),    # several pixels per cell, mirror boundary on all sides
+    (2, 33, 47, 5, 3, 4, 3, 4, False),   # no offset
+    (1, 16, 16, 2, 2, 1, 1, 1, True),    # gd = 1: both depth borders at once
+]
+
+# (B, H, W, gh, gw, gd, gc)
+SLICE_CASES = [(3, 30, 25, 16, 12, 8, 12), (2, 21, 36, 5, 4, 6, 2), (1, 9, 7, 3, 3, 9, 5)]
+
+
 def rand_case(seed, B, H, W, gh, gw, gd, n_in=3, n_out=3, has_offset=True, signed=False):
     """Seeded inputs as the reference's tests draw them (np.random.rand; hdrnet_ops_test.py:101)."""
     rng = np.random.RandomState(seed)

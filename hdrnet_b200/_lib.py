@@ -63,7 +63,15 @@ SIGNATURES = {
     "hdrnet_conv2d_nhwc_tc_f32": (_c_int, [_vp] * 4 + [_c_int] * 8 + [_vp]),
     "hdrnet_fc_f32": (_c_int, [_vp] * 4 + [_c_int] * 4 + [_vp]),
     "hdrnet_fuse_predict_f32": (_c_int, [_vp] * 5 + [_c_int] * 7 + [_vp]),
-    "hdrnet_resize_bilinear_f32": (_c_int, [_vp] * 3 + [_c_int] * 6 + [_vp]),
+    # (in, w, out, dout, din, dw, db, B,H,W,Cin,Cout,k,stride,relu, ws, bytes, stream)
+    "hdrnet_conv2d_grad_workspace_bytes": (ctypes.c_size_t, [_c_int] * 7),
+    "hdrnet_conv2d_grad_f32": (_c_int, [_vp] * 7 + [_c_int] * 8 + [_vp, ctypes.c_size_t, _vp]),
+    "hdrnet_fc_grad_workspace_bytes": (ctypes.c_size_t, [_c_int] * 3),
+    "hdrnet_fc_grad_f32": (_c_int, [_vp] * 7 + [_c_int] * 4 + [_vp, ctypes.c_size_t, _vp]),
+    # (local, global, w, dgrid, dlocal, dglobal, dw, db, B,gh,gw,C,gd,n_out,n_in, ws, bytes, stream)
+    "hdrnet_fuse_predict_grad_workspace_bytes": (ctypes.c_size_t, [_c_int] * 7),
+    "hdrnet_fuse_predict_grad_f32": (_c_int, [_vp] * 8 + [_c_int] * 7 + [_vp, ctypes.c_size_t, _vp]),
+    "hdrnet_resize_bilinear_f32":(_c_int, [_vp] * 3 + [_c_int] * 6 + [_vp]),
     "hdrnet_coefficients_scratch_bytes": (ctypes.c_size_t, [_c_int] * 7),
     "hdrnet_coefficients_f32": (_c_int, [_vp] * 4 + [_c_int, _vp, ctypes.c_size_t] + [_c_int] * 7 + [_vp]),
     "hdrnet_host_ctx_create": (_c_int, [ctypes.POINTER(_vp), ctypes.c_size_t]),

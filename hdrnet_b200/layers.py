@@ -14,8 +14,11 @@ Same names, argument order and shapes as the reference (hdrnet/layers.py:99-198)
 the layer's variables under ``scope``; here the variables already exist -- a dict keyed by the
 reference's variable names (``<scope>/weights``, ``<scope>/biases``, ``<scope>/BatchNorm/beta`` ...;
 ``weights=`` or the dict given to ``models.set_weights``) -- and ``scope`` is the full variable scope
-(e.g. ``inference/coefficients/splat/conv1``).  The models call the same kernels through
-``hdrnet_b200.models`` with device-resident, pre-folded weights.
+(e.g. ``inference/coefficients/splat/conv1``).  The variables may be CUDA float32 tensors: with
+grad enabled and the input or a variable requiring grad, the layer is an autograd Function whose
+backward runs the VJP kernels (csrc/cnn_grad.cu); batch-norm layers are not differentiated.
+The models call the same kernels through ``hdrnet_b200.models`` with device-resident, pre-folded
+weights.
 """
 from __future__ import annotations
 
@@ -37,9 +40,25 @@ def _layer_variables(scope, weights, use_bias, batch_norm, device):
     if scope is None:
         raise ValueError("scope is required: it names the layer's variables (<scope>/weights, ...)")
     wts = weights if weights is not None else models._resolve_weights({})
-    w, b = models._fold(wts, scope, bool(batch_norm), bool(use_bias))
+    if not batch_norm and isinstance(wts.get(scope + "/weights"), torch.Tensor):
+        # tensor variables are used as they are, so that gradients reach them
+        wd = models._device_var(wts[scope + "/weights"], device)
+        return wd, (models._device_var(wts[scope + "/biases"], device) if use_bias else None)
+    host = models._HostView(wts) if models._has_tensors(wts) else wts
+    w, b = models._fold(host, scope, bool(batch_norm), bool(use_bias))
     wd = torch.from_numpy(w).contiguous().to(device)
     return wd, (None if b is None else torch.from_numpy(b).contiguous().to(device))
+
+
+def _refuse_batch_norm(scope, weights, batch_norm) -> None:
+    from . import models
+    wts = weights if weights is not None else models._weights
+    if batch_norm and scope is not None and wts is not None:
+        models._refuse_batch_norm_scope(wts, scope)
+
+
+def _differentiable(*ts) -> bool:
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
 
 
 def _activation(activation_fn):
@@ -66,6 +85,7 @@ def conv(inputs: torch.Tensor, num_outputs: int, kernel_size: int, stride: int =
     from . import models
     if is_training:
         raise NotImplementedError("hdrnet_b200 implements the inference path only")
+    _refuse_batch_norm(scope, weights, batch_norm)
     if rate != 1:
         raise NotImplementedError("dilated convolutions (rate != 1) are not used by the reference models")
     if not isinstance(inputs, torch.Tensor) or inputs.dtype != torch.float32 or inputs.dim() != 4:
@@ -79,7 +99,10 @@ def conv(inputs: torch.Tensor, num_outputs: int, kernel_size: int, stride: int =
                          f"[{kernel_size}, {kernel_size}, Cin, {num_outputs}]")
     fused, post = _activation(activation_fn)
     with torch.cuda.device(inputs.device):
-        out = models._conv(inputs.contiguous(), (w, b), stride=stride, relu=fused)
+        if _differentiable(inputs, w, b):
+            out = models._ConvFn.apply(inputs, w, b, stride, fused, False)
+        else:
+            out = models._conv(inputs.contiguous(), (w, b), stride=stride, relu=fused)
     return out if post is None else post(out)
 
 
@@ -91,6 +114,7 @@ def fc(inputs: torch.Tensor, num_outputs: int, use_bias: bool = True, batch_norm
     from . import models
     if is_training:
         raise NotImplementedError("hdrnet_b200 implements the inference path only")
+    _refuse_batch_norm(scope, weights, batch_norm)
     if not isinstance(inputs, torch.Tensor) or inputs.dtype != torch.float32 or inputs.dim() != 2:
         raise ValueError("inputs must be a float32 tensor [B, I]")
     if inputs.device.type != "cuda":
@@ -101,7 +125,10 @@ def fc(inputs: torch.Tensor, num_outputs: int, use_bias: bool = True, batch_norm
         raise ValueError(f"{scope}/weights has shape {tuple(w.shape)}, expected [I, {num_outputs}]")
     fused, post = _activation(activation_fn)
     with torch.cuda.device(inputs.device):
-        out = models._fc(inputs.contiguous(), (w, b), relu=fused)
+        if _differentiable(inputs, w, b):
+            out = models._FcFn.apply(inputs, w, b, fused)
+        else:
+            out = models._fc(inputs.contiguous(), (w, b), relu=fused)
     return out if post is None else post(out)
 
 

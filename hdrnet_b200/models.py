@@ -16,6 +16,16 @@ flat dict of numpy arrays keyed by the SAME variable names under ``inference/``
 install it once with ``set_weights`` / ``load_weights``.  Conv weights are HWIO, FC weights
 [in, out], exactly as TF stores them.
 
+The values may also be CUDA float32 ``torch.Tensor``s.  With grad enabled and any coefficient-network
+variable (or ``lowres_input``) requiring grad, ``_coefficients`` runs layer by layer through
+autograd Functions over the same forward kernels and the VJP kernels of ``csrc/cnn_grad.cu``, so
+``torch.optim`` can fine-tune the network through the slice-apply VJP with the guide held fixed.
+A dict holding tensors is never cached: every call reads the current values.  The gradients are
+those of the inference-form graph; with ``batch_norm=False`` (the reference's default,
+hdrnet/bin/train.py:224-236) that is the coefficient network's training graph.  Guide variables,
+``fullres_input``, batch-norm layers and the pyramid model's resize are not differentiated: asking
+for their gradient raises ``NotImplementedError``.
+
 Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
   coefficients  4 splat convs, 2 global convs + 3 FCs, 2 local convs (conv2d / fc kernels),
                 then fusion + prediction + unroll_grid in one kernel -> grid [B,gh,gw,gd,12]
@@ -69,6 +79,11 @@ def _resolve_weights(params) -> dict:
     if w is None:
         raise ValueError("no weights: pass params['weights'] or call models.set_weights()")
     return w
+
+
+def _weights_or_none(params):
+    w = params.get("weights") if isinstance(params, dict) else None
+    return _weights if w is None else w
 
 
 def init_weights(params, seed: int = 0, model_name: str | None = None) -> dict:
@@ -182,27 +197,65 @@ def _fold(wts, scope, use_bn, use_bias):
     return w, None
 
 
+def _has_tensors(wts) -> bool:
+    return any(isinstance(v, torch.Tensor) for v in wts.values())
+
+
+class _HostView:
+    """Read-only view of a weights dict with tensor values as host numpy arrays (for _fold and the
+    guide parameters, which the kernels take as host arrays)."""
+
+    def __init__(self, wts):
+        self._wts = wts
+
+    def __getitem__(self, key):
+        v = self._wts[key]
+        return v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v
+
+
+def _device_var(v, device) -> torch.Tensor:
+    """A variable as a contiguous float32 tensor on `device`: a tensor already there is used as is
+    (it keeps its autograd identity), anything else is copied."""
+    if isinstance(v, torch.Tensor):
+        return v.to(device=device, dtype=torch.float32).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(np.asarray(v, np.float32))).to(device)
+
+
+def _coefficient_specs(params):
+    """(scope, batch norm, bias) of every coefficient-network layer, in network order."""
+    bn = bool(params["batch_norm"])
+    p = "inference/coefficients"
+    n_ds = int(np.log2(params["net_input_size"] / params["spatial_bin"]))
+    specs = [(f"{p}/splat/conv{i + 1}", bn and i > 0, True) for i in range(n_ds)]
+    specs += [(f"{p}/global/conv1", bn, True), (f"{p}/global/conv2", bn, True),
+              (f"{p}/global/fc1", bn, True), (f"{p}/global/fc2", bn, True),
+              (f"{p}/global/fc3", False, True), (f"{p}/local/conv1", bn, True),
+              (f"{p}/local/conv2", False, False), (f"{p}/prediction/conv1", False, True)]
+    return specs
+
+
 class _Prepared:
     """Device copies of the coefficient-network weights + host copies of the guide params."""
 
     def __init__(self, wts, params, device, nn_guide):
         self.device = device
         self.source = wts   # keeps the dict alive: the cache is keyed by id(wts)
-        bn = bool(params["batch_norm"])
         self.layers = {}
-        p = "inference/coefficients"
-        n_ds = int(np.log2(params["net_input_size"] / params["spatial_bin"]))
-        specs = [(f"{p}/splat/conv{i + 1}", bn and i > 0, True) for i in range(n_ds)]
-        specs += [(f"{p}/global/conv1", bn, True), (f"{p}/global/conv2", bn, True),
-                  (f"{p}/global/fc1", bn, True), (f"{p}/global/fc2", bn, True),
-                  (f"{p}/global/fc3", False, True), (f"{p}/local/conv1", bn, True),
-                  (f"{p}/local/conv2", False, False), (f"{p}/prediction/conv1", False, True)]
-        for scope, use_bn, use_bias in specs:
-            w, b = _fold(wts, scope, use_bn, use_bias)
-            wd = torch.from_numpy(np.ascontiguousarray(w)).to(device)
-            bd = None if b is None else torch.from_numpy(np.ascontiguousarray(b)).to(device)
-            packed = pack_conv_weights(wd) if (wd.dim() == 4 and device.type == "cuda") else None
+        tensors = _has_tensors(wts)
+        host = _HostView(wts) if tensors else wts
+        for scope, use_bn, use_bias in _coefficient_specs(params):
+            if tensors and not use_bn:
+                # the variables themselves (no copy when they are CUDA float32 already)
+                wd = _device_var(wts[scope + "/weights"], device)
+                bd = _device_var(wts[scope + "/biases"], device) if use_bias else None
+            else:
+                w, b = _fold(host, scope, use_bn, use_bias)
+                wd = torch.from_numpy(np.ascontiguousarray(w)).to(device)
+                bd = None if b is None else torch.from_numpy(np.ascontiguousarray(b)).to(device)
+            # tensor variables change between optimizer steps: packed per call (this object is)
+            packed = pack_conv_weights(wd.detach()) if (wd.dim() == 4 and device.type == "cuda") else None
             self.layers[scope] = (wd, bd, packed)
+        wts = host
         g = "inference/guide"
         f32 = lambda a: np.ascontiguousarray(np.asarray(a, np.float32))  # noqa: E731
 
@@ -226,6 +279,9 @@ class _Prepared:
 
 
 def _prepare(wts, params, device, nn_guide) -> _Prepared:
+    if _has_tensors(wts):
+        # tensor variables may be updated in place (optimizer steps): never served from the cache
+        return _Prepared(wts, params, device, nn_guide)
     key = (id(wts), str(device), str(nn_guide), bool(params["batch_norm"]),
            params["net_input_size"], params["spatial_bin"])
     prep = _prepared.get(key)
@@ -365,6 +421,190 @@ def _fc(x: torch.Tensor, wb, relu=True) -> torch.Tensor:
     return out
 
 
+# ---- autograd over the layer kernels (backward: csrc/cnn_grad.cu) ------------------------------
+def _stream(device):
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def _grad_workspace(device, nbytes: int) -> torch.Tensor:
+    """Partial-sum workspace of one VJP call, lent to the library (it never allocates)."""
+    return torch.empty((max(int(nbytes), 16) + 3) // 4, dtype=torch.float32, device=device)
+
+
+def _ptr(t) -> int:
+    return 0 if t is None else t.data_ptr()
+
+
+class _ConvFn(torch.autograd.Function):
+    """One conv layer (hdrnet/layers.py:25-59, inference batch norm already folded): forward
+    hdrnet_conv2d_nhwc_f32 / its tensor-core form, backward hdrnet_conv2d_grad_f32."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, stride, relu, tc=True):
+        x, w = x.contiguous(), w.contiguous()
+        b = None if b is None else b.contiguous()
+        B, H, W, _ = x.shape
+        oh, ow = -(-H // stride), -(-W // stride)
+        # tc: the packed tensor-core form where _conv would take it (the model path; layers.conv
+        # never packs).  The variables change between optimizer steps, so they are packed per call.
+        packed = pack_conv_weights(w) if (tc and _use_packed_tc((B * oh * ow + 127) // 128)) else None
+        with torch.cuda.device(x.device):
+            out = _conv(x, (w, b, packed), stride=stride, relu=relu)
+        ctx.save_for_backward(x, w, out)
+        ctx.stride, ctx.relu, ctx.has_bias = stride, bool(relu), b is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, out = ctx.saved_tensors
+        dy = dy.contiguous()
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        B, H, W, cin = x.shape
+        k, cout = w.shape[0], w.shape[3]
+        dx = torch.empty_like(x) if need_x else None
+        dw = torch.empty_like(w) if need_w else None
+        db = torch.empty(cout, dtype=torch.float32, device=x.device) if (need_b and ctx.has_bias) else None
+        lib = _lib.load()
+        ws = None
+        if dw is not None or db is not None:
+            ws = _grad_workspace(x.device, lib.hdrnet_conv2d_grad_workspace_bytes(B, H, W, cin, cout, k, ctx.stride))
+        with torch.cuda.device(x.device):
+            rc = lib.hdrnet_conv2d_grad_f32(
+                x.data_ptr(), w.data_ptr(), out.data_ptr(), dy.data_ptr(), _ptr(dx), _ptr(dw), _ptr(db),
+                B, H, W, cin, cout, k, ctx.stride, int(ctx.relu), _ptr(ws),
+                0 if ws is None else ws.numel() * 4, _stream(x.device))
+        _lib.check(rc, "conv2d VJP")
+        return dx, dw, db, None, None, None
+
+
+class _FcFn(torch.autograd.Function):
+    """One fully connected layer (hdrnet/layers.py:62-93): forward hdrnet_fc_f32, backward
+    hdrnet_fc_grad_f32."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, relu):
+        x, w = x.contiguous(), w.contiguous()
+        b = None if b is None else b.contiguous()
+        with torch.cuda.device(x.device):
+            out = _fc(x, (w, b), relu=relu)
+        ctx.save_for_backward(x, w, out)
+        ctx.relu, ctx.has_bias = bool(relu), b is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, out = ctx.saved_tensors
+        dy = dy.contiguous()
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        B, I = x.shape
+        O = w.shape[1]
+        dx = torch.empty_like(x) if need_x else None
+        dw = torch.empty_like(w) if need_w else None
+        db = torch.empty(O, dtype=torch.float32, device=x.device) if (need_b and ctx.has_bias) else None
+        lib = _lib.load()
+        ws = None
+        if dw is not None or db is not None:
+            ws = _grad_workspace(x.device, lib.hdrnet_fc_grad_workspace_bytes(B, I, O))
+        with torch.cuda.device(x.device):
+            rc = lib.hdrnet_fc_grad_f32(
+                x.data_ptr(), w.data_ptr(), out.data_ptr(), dy.data_ptr(), _ptr(dx), _ptr(dw), _ptr(db),
+                B, I, O, int(ctx.relu), _ptr(ws), 0 if ws is None else ws.numel() * 4, _stream(x.device))
+        _lib.check(rc, "fc VJP")
+        return dx, dw, db, None
+
+
+class _FusePredictFn(torch.autograd.Function):
+    """Fusion + prediction + unroll_grid (models.py:122-139): forward hdrnet_fuse_predict_f32,
+    backward hdrnet_fuse_predict_grad_f32 (fused = relu(local + global) is recomputed there from the
+    saved local and global)."""
+
+    @staticmethod
+    def forward(ctx, local, glob, w, b, gd, n_out, n_in):
+        local, glob, w = local.contiguous(), glob.contiguous(), w.contiguous()
+        b = None if b is None else b.contiguous()
+        bs, gh, gw, C = local.shape
+        grid = torch.empty((bs, gh, gw, gd, n_out, n_in), dtype=torch.float32, device=local.device)
+        with torch.cuda.device(local.device):
+            rc = _lib.load().hdrnet_fuse_predict_f32(
+                local.data_ptr(), glob.data_ptr(), w.data_ptr(), _ptr(b), grid.data_ptr(), bs, gh, gw,
+                C, gd, n_out, n_in, _stream(local.device))
+        _lib.check(rc, "fuse_predict")
+        ctx.save_for_backward(local, glob, w)
+        ctx.dims, ctx.has_bias = (gd, n_out, n_in), b is not None
+        return grid
+
+    @staticmethod
+    def backward(ctx, dgrid):
+        local, glob, w = ctx.saved_tensors
+        dgrid = dgrid.contiguous()
+        gd, n_out, n_in = ctx.dims
+        need_l, need_g, need_w, need_b = ctx.needs_input_grad[:4]
+        bs, gh, gw, C = local.shape
+        dl = torch.empty_like(local) if need_l else None
+        dg = torch.empty_like(glob) if need_g else None
+        dw = torch.empty_like(w) if need_w else None
+        db = torch.empty(w.shape[1], dtype=torch.float32, device=w.device) if (need_b and ctx.has_bias) else None
+        lib = _lib.load()
+        ws = None
+        if dw is not None or db is not None:
+            ws = _grad_workspace(local.device, lib.hdrnet_fuse_predict_grad_workspace_bytes(
+                bs, gh, gw, C, gd, n_out, n_in))
+        with torch.cuda.device(local.device):
+            rc = lib.hdrnet_fuse_predict_grad_f32(
+                local.data_ptr(), glob.data_ptr(), w.data_ptr(), dgrid.data_ptr(), _ptr(dl), _ptr(dg),
+                _ptr(dw), _ptr(db), bs, gh, gw, C, gd, n_out, n_in, _ptr(ws),
+                0 if ws is None else ws.numel() * 4, _stream(local.device))
+        _lib.check(rc, "fuse_predict VJP")
+        return dl, dg, dw, db, None, None, None
+
+
+def _requires_grad(t) -> bool:
+    return isinstance(t, torch.Tensor) and t.requires_grad
+
+
+def _trainable_keys(wts, prefix: str):
+    return sorted(k for k, v in wts.items() if k.startswith(prefix) and _requires_grad(v))
+
+
+def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None) -> None:
+    """NotImplementedError for every gradient this package does not compute (checked before any
+    device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN)."""
+    if not torch.is_grad_enabled() or wts is None:
+        return
+    if what is not None:
+        wanted = _trainable_keys(wts, "inference/") + \
+            [n for n, t in (("lowres_input", lowres_input), ("fullres_input", fullres_input)) if _requires_grad(t)]
+        if wanted:
+            raise NotImplementedError(f"{what}: gradients are not implemented (requested for {wanted[0]}); "
+                                      "its _coefficients is differentiable on its own")
+        return
+    guide = _trainable_keys(wts, "inference/guide")
+    if guide:
+        raise NotImplementedError(f"gradients for the guide variables are not implemented ({guide[0]} requires "
+                                  "grad): the guide is held fixed; set requires_grad=False on its variables")
+    if _requires_grad(fullres_input):
+        raise NotImplementedError("gradients for fullres_input are not implemented: they need the guide's "
+                                  "backward; pass it with requires_grad=False")
+    _refuse_batch_norm(wts, params)
+
+
+def _refuse_batch_norm(wts, params) -> None:
+    if not torch.is_grad_enabled() or wts is None:
+        return
+    for scope, use_bn, _ in _coefficient_specs(params):
+        if use_bn:
+            _refuse_batch_norm_scope(wts, scope)
+
+
+def _refuse_batch_norm_scope(wts, scope) -> None:
+    """A batch-norm layer is folded in its inference form: its variables get no gradient."""
+    keys = _trainable_keys(wts, scope + "/") if torch.is_grad_enabled() else []
+    if keys:
+        raise NotImplementedError(
+            f"gradients through a batch-norm layer are not implemented ({keys[0]} requires grad): "
+            "training-mode batch norm uses batch statistics, a different forward")
+
+
 class HDRNetCurves(object):
     """Main model, as submitted in January 2017 (hdrnet/models.py:30-196)."""
 
@@ -382,11 +622,21 @@ class HDRNetCurves(object):
     def inference(cls, lowres_input, fullres_input, params, is_training=False):
         """models.py:43-59.  lowres_input [B,S,S,3], fullres_input [B,H,W,3] -> [B,H,W,3].
         With params['debug'] truthy also stores the coefficients and guide on
-        ``cls.last_debug`` (the collections run.py --debug reads, run.py:98-133)."""
+        ``cls.last_debug`` (the collections run.py --debug reads, run.py:98-133).
+
+        With coefficient-network variables (or lowres_input) requiring grad, the coefficients come
+        from autograd and the output from the standalone guide kernel (a constant) and
+        hdrnet_ops.bilateral_slice_apply, whose VJP carries the gradient back to the grid."""
         if is_training:
             raise NotImplementedError("hdrnet_b200 implements the inference path only")
+        _refuse_untrained(_weights_or_none(params), params, fullres_input=fullres_input)
         fullres_input = _check_input(fullres_input, "fullres_input")
         coeffs = cls._coefficients(lowres_input, params, is_training)
+        if coeffs.requires_grad:
+            with torch.cuda.device(fullres_input.device):
+                guide = cls._guide(fullres_input, params)
+            B, gh, gw, gd = coeffs.shape[:4]
+            return bilateral_slice_apply(coeffs.reshape(B, gh, gw, gd, -1), guide, fullres_input, True)
         return cls._fullres(coeffs, fullres_input, params, torch.float32)
 
     @classmethod
@@ -466,6 +716,7 @@ class HDRNetCurves(object):
         """models.py:62-142 -> [B, gh, gw, gd, n_out, n_in]."""
         if is_training:
             raise NotImplementedError("hdrnet_b200 implements the inference path only")
+        _refuse_batch_norm(_weights_or_none(params), params)
         x = _check_input(input_tensor, "lowres_input")
         prep = _prepare(_resolve_weights(params), params, x.device, cls._nn_guide)
         L = prep.layers
@@ -473,6 +724,9 @@ class HDRNetCurves(object):
         p = "inference/coefficients"
         n_ds = int(np.log2(params["net_input_size"] / params["spatial_bin"]))
         bs = x.shape[0]
+        if torch.is_grad_enabled() and (x.requires_grad or any(
+                _requires_grad(t) for wb in L.values() for t in wb[:2])):
+            return cls._coefficients_autograd(x, L, gd, n_ds)
         # small batches: the whole network behind one library call (launch chain, csrc/cnn.cu)
         if bs <= CHAIN_CNN_MAX_BATCH and os.environ.get("HDRNET_CONV_TCGEN05") != "1":
             grid = cls._coefficients_chain(x, prep, params, n_ds)
@@ -500,6 +754,27 @@ class HDRNetCurves(object):
                 torch.cuda.current_stream(x.device).cuda_stream)
         _lib.check(rc, "fuse_predict")
         return grid
+
+    @classmethod
+    def _coefficients_autograd(cls, x, L, gd, n_ds):
+        """The per-layer path above with every layer an autograd Function: the same kernels in the
+        same order (so the same values, bitwise), and a backward through csrc/cnn_grad.cu."""
+        p = "inference/coefficients"
+        bs = x.shape[0]
+        with torch.cuda.device(x.device):
+            for i in range(n_ds):
+                x = _ConvFn.apply(x, *L[f"{p}/splat/conv{i + 1}"][:2], 2, True)
+            splat = x
+            g = _ConvFn.apply(splat, *L[f"{p}/global/conv1"][:2], 2, True)
+            g = _ConvFn.apply(g, *L[f"{p}/global/conv2"][:2], 2, True)
+            g = g.reshape(bs, -1)
+            g = _FcFn.apply(g, *L[f"{p}/global/fc1"][:2], True)
+            g = _FcFn.apply(g, *L[f"{p}/global/fc2"][:2], True)
+            g = _FcFn.apply(g, *L[f"{p}/global/fc3"][:2], False)
+            loc = _ConvFn.apply(splat, *L[f"{p}/local/conv1"][:2], 1, True)
+            loc = _ConvFn.apply(loc, *L[f"{p}/local/conv2"][:2], 1, False)
+            wp, bp = L[f"{p}/prediction/conv1"][:2]                 # HWIO [1, 1, C, O] -> [C, O]
+            return _FusePredictFn.apply(loc, g, wp.reshape(wp.shape[-2:]), bp, gd, cls.n_out(), cls.n_in())
 
     @classmethod
     def _coefficients_chain(cls, x, prep, params, n_ds):
@@ -613,6 +888,8 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
     def inference(cls, lowres_input, fullres_input, params, is_training=False):
         if is_training:
             raise NotImplementedError("hdrnet_b200 implements the inference path only")
+        _refuse_untrained(_weights_or_none(params), params, lowres_input, fullres_input,
+                          what="HDRNetGaussianPyrNN.inference (needs the VJP of the align-corners resize)")
         fullres_input = _check_input(fullres_input, "fullres_input")
         coeffs = cls._coefficients(lowres_input, params, is_training)       # [B,gh,gw,gd,9,4]
         with torch.cuda.device(fullres_input.device):

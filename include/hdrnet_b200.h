@@ -269,6 +269,51 @@ HDRNET_API int hdrnet_fuse_predict_f32(const float* local, const float* global_f
                                        void* stream);
 
 /*
+ * Vector-Jacobian products of the coefficient network's layers (fine-tuning the network through
+ * the slice-apply VJP; the backward of hdrnet/models.py:62-142 that TF's gradients give).  Same
+ * layouts and the same TF 'SAME' geometry as the forwards above.  `dout` is the gradient of the
+ * layer's output; for a ReLU layer it is masked by `out > 0` (TF's ReluGrad masks on the layer's
+ * output), so `out` is required when relu != 0 and may be NULL otherwise.  Any of din / dw / db
+ * may be NULL when that gradient is not wanted (din of the first layer, db of a layer without
+ * bias); `w` may be NULL when din is, `in` when dw and db are.  Gradients are written, not
+ * accumulated.  The weight and bias VJPs sum over output pixels in per-CTA chunks whose partial
+ * sums go to a caller-lent workspace (*_workspace_bytes; the library never allocates), then a
+ * second pass adds the chunks in a fixed order.  No floating-point atomics: results are
+ * bitwise reproducible.  The workspace is scratch, undefined after the call.
+ *
+ * conv2d VJP: the backward of hdrnet_conv2d_nhwc_f32 (and of its tensor-core form).
+ */
+HDRNET_API size_t hdrnet_conv2d_grad_workspace_bytes(int B, int H, int W, int Cin, int Cout, int k,
+                                                     int stride);
+HDRNET_API int hdrnet_conv2d_grad_f32(const float* in, const float* w, const float* out,
+                                      const float* dout, float* din, float* dw, float* db, int B,
+                                      int H, int W, int Cin, int Cout, int k, int stride, int relu,
+                                      void* workspace, size_t workspace_bytes, void* stream);
+
+/* fully_connected VJP: the backward of hdrnet_fc_f32 (din = dout' w^T, dw = in^T dout',
+ * db = sum_b dout'). */
+HDRNET_API size_t hdrnet_fc_grad_workspace_bytes(int B, int I, int O);
+HDRNET_API int hdrnet_fc_grad_f32(const float* in, const float* w, const float* out,
+                                  const float* dout, float* din, float* dw, float* db, int B, int I,
+                                  int O, int relu, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+
+/*
+ * Fusion + prediction + unroll_grid VJP: the backward of hdrnet_fuse_predict_f32.  dgrid has the
+ * grid's shape; dpred[o] = dgrid[b,y,x,z,i,j] for o = (j*n_out + i)*gd + z.  fused =
+ * relu(local + global) is recomputed from the saved local / global, not stored:
+ *   dw[c][o] = sum_{b,y,x} fused * dpred,  db[o] = sum dpred,
+ *   dlocal = (dpred w^T) * (fused > 0),   dglobal[b,c] = sum_{y,x} dlocal[b,y,x,c].
+ */
+HDRNET_API size_t hdrnet_fuse_predict_grad_workspace_bytes(int B, int gh, int gw, int C, int gd,
+                                                           int n_out, int n_in);
+HDRNET_API int hdrnet_fuse_predict_grad_f32(const float* local, const float* global_feat,
+                                            const float* w, const float* dgrid, float* dlocal,
+                                            float* dglobal, float* dw, float* db, int B, int gh,
+                                            int gw, int C, int gd, int n_out, int n_in,
+                                            void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * The WHOLE coefficient network (splat convs, global convs + fcs, local convs, fusion, prediction,
  * unroll_grid) behind one call: replaces HDRNetCurves._coefficients, hdrnet/models.py:62-142, with
  * batch norm folded by the caller.  At small batch the twelve layers are 8 launches -- the global

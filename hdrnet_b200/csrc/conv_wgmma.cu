@@ -405,6 +405,8 @@ int hdrnet_conv2d_tc_pack_f32(const float* w, float* packed, int k, int Cin, int
                               void* stream) {
   if (hdrnet_conv2d_tc_packed_bytes(k, Cin, Cout) == 0) return HDRNET_E_UNSUPPORTED;
   if (!w || !packed) return HDRNET_E_NULL_POINTER;
+  // the pack kernel stores float4s into `packed` (and the layer call bulk-copies from it)
+  if (reinterpret_cast<uintptr_t>(packed) & 15u) return HDRNET_E_UNSUPPORTED;
   const int K = k * k * Cin, nchunks = (K + kTcKc - 1) / kTcKc;
   const long long total = static_cast<long long>(nchunks) * 8 * Cout;
   conv_tc_pack_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0,

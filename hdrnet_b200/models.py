@@ -325,6 +325,14 @@ def _check_image(t: torch.Tensor, what: str) -> torch.Tensor:
     return t.contiguous()
 
 
+def _fused_row_kernel_takes(W: int, *bufs: torch.Tensor) -> bool:
+    """Whether the float32 guide-fused slice-apply can run without a guide buffer: its row kernel
+    takes W % 4 == 0, W >= 128 and 16-byte aligned buffers (include/hdrnet_b200.h); anything else
+    runs the guide kernel into the caller's buffer first.  A contiguous view at an offset (a frame
+    carved out of a packed buffer, an ``out`` from a pool) is not aligned."""
+    return W % 4 == 0 and W >= 128 and all(t.data_ptr() % 16 == 0 for t in bufs)
+
+
 def lowres_from_image(image: torch.Tensor, size: int) -> torch.Tensor:
     """[B,H,W,3] uint8 / uint16 / float32 -> [B,size,size,3] float32: img_as_float +
     skimage.transform.resize(order=0) of hdrnet/bin/run.py:156-169 in one gather kernel."""
@@ -680,8 +688,8 @@ class HDRNetCurves(object):
         out = torch.empty((B, H, W, 3), dtype=out_dtype, device=fullres_input.device)
         debug = bool(params.get("debug"))
         f32 = in_fmt == _lib.PX_F32 and out_fmt == _lib.PX_F32
-        # the float32 form needs the guide buffer for shapes its row kernel cannot take
-        need_guide = debug or (f32 and ((W % 4 != 0) or W < 128))
+        # the float32 form needs the guide buffer for shapes and buffers its row kernel cannot take
+        need_guide = debug or (f32 and not _fused_row_kernel_takes(W, fullres_input, out, coeffs))
         guide = torch.empty((B, H, W), dtype=torch.float32, device=fullres_input.device) \
             if need_guide else None
         lib = _lib.load()
@@ -957,7 +965,7 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
             else:
                 w1, b1, w2, b2, feats = prep.nn_levels[src]
                 out_lvl = torch.empty_like(lvl)
-                need_guide = (W % 4 != 0) or W < 128
+                need_guide = not _fused_row_kernel_takes(W, lvl, out_lvl, c)
                 scratch = torch.empty((B, H, W), dtype=torch.float32, device=lvl.device) \
                     if need_guide else None
                 rc = lib.hdrnet_slice_apply_nn_f32(

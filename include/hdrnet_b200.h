@@ -241,8 +241,9 @@ HDRNET_API int hdrnet_conv2d_nhwc_f32(const float* in, const float* w, const flo
 /*
  * Tensor-core form of conv2d (wgmma.mma_async .tf32 with 3xTF32 operand splitting, fp32
  * accumulator; float32-grade results).  Weights are packed ONCE per model into per-chunk hi/lo tiles
- * in the MMA's shared-memory layout (hdrnet_conv2d_tc_packed_bytes() bytes, device memory owned
- * by the caller); the layer call then needs Cin % 4 == 0, Cout % 16 == 0, 16 <= Cout <= 128.
+ * in the MMA's shared-memory layout (hdrnet_conv2d_tc_packed_bytes() bytes, 16-byte aligned device
+ * memory owned by the caller: HDRNET_E_UNSUPPORTED otherwise); the layer call then needs
+ * Cin % 4 == 0, Cout % 16 == 0, 16 <= Cout <= 128.
  * hdrnet_conv2d_nhwc_f32 also reaches an unpacked tensor-core kernel on its own when the layer
  * has >= 96 tiles of 128 pixels (HDRNET_CONV_TCGEN05=0/1 overrides).
  */

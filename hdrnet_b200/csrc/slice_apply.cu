@@ -772,6 +772,15 @@ static int device_max_smem_optin() {
   return v;
 }
 
+// Base alignment a texture object over linear memory needs (512 bytes on H100): the texture-assisted
+// forms fetch the slab workspace through one, and cudaCreateTextureObject refuses other bases.
+static int device_texture_alignment() {
+  int dev = 0, v = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 512;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrTextureAlignment, dev) != cudaSuccess) return 512;
+  return v > 0 ? v : 512;
+}
+
 
 // Returns false when the TMA kernel cannot run these shapes.
 // tex_mode: the texture-assisted form double-buffers whole slab rows in raw0 / raw1 and needs no
@@ -925,7 +934,10 @@ static int get_slab_texture(const float* ws, size_t bytes, cudaTextureObject_t* 
   td.readMode = cudaReadModeElementType;
   cudaTextureObject_t tex = 0;
   cudaError_t err = cudaCreateTextureObject(&tex, &rd, &td, nullptr);
-  if (err != cudaSuccess) return static_cast<int>(err);
+  if (err != cudaSuccess) {
+    (void)cudaGetLastError();   // report it from this call only: the next launch's check must not see it
+    return static_cast<int>(err);
+  }
   cudaEvent_t ev = nullptr;
   err = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
   if (err != cudaSuccess) { cudaDestroyTextureObject(tex); return static_cast<int>(err); }
@@ -1039,7 +1051,8 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
   // Texture-assisted forms: possible when the caller lent a workspace for the slab rows.
   const size_t tex_need = row_shape ? static_cast<size_t>(B) * rows * plan.row_floats * sizeof(float) : 0;
   const bool tex_ok = row_shape && gs.workspace && gs.workspace_bytes >= tex_need &&
-                      aligned16(gs.workspace) && gs.workspace_bytes / 16 <= (1u << 27);
+                      reinterpret_cast<uintptr_t>(gs.workspace) % device_texture_alignment() == 0 &&
+                      gs.workspace_bytes / 16 <= (1u << 27);
   // Issuer-warp form: float32 pixels, guide as an input, a ring of >= 3 stages at two CTAs per SM.
   TmaPlan aplan;
   bool async_ok = tex_ok && gs.mode == 0 && !px &&

@@ -93,7 +93,10 @@ HDRNET_API int hdrnet_slice_apply_f32_variant(const float* grid, const float* gu
 /*
  * Same op with a caller-provided device workspace (the library itself never allocates):
  * required by HDRNET_VARIANT_TEX, ignored by the other variants.
- * hdrnet_slice_apply_workspace_bytes() = B * H * gw * gd * 48.
+ * hdrnet_slice_apply_workspace_bytes() = B * H * gw * gd * 48.  The texture-assisted forms read
+ * the workspace through a texture object, so they need it aligned to the device's texture alignment
+ * (512 bytes on H100; cudaMalloc and torch's allocator return such blocks): with any other base AUTO
+ * runs the TMA row kernel and a forced TEX / TEX_ASYNC returns HDRNET_E_UNSUPPORTED.
  * The workspace is scratch: its contents are undefined after a call (the kernels may drop rows
  * they are done with from L2 without writing them back), and a call never reads what an earlier
  * call left there.

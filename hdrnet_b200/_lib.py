@@ -74,6 +74,8 @@ SIGNATURES = {
     "hdrnet_resize_bilinear_f32":(_c_int, [_vp] * 3 + [_c_int] * 6 + [_vp]),
     "hdrnet_coefficients_scratch_bytes": (ctypes.c_size_t, [_c_int] * 7),
     "hdrnet_coefficients_f32": (_c_int, [_vp] * 4 + [_c_int, _vp, ctypes.c_size_t] + [_c_int] * 7 + [_vp]),
+    # (samples, B, fullres_in, fullres_out, lowres_in, oh, ow, S, stream)
+    "hdrnet_train_batch_f32": (_c_int, [_vp, _c_int] + [_vp] * 3 + [_c_int] * 3 + [_vp]),
     "hdrnet_host_ctx_create": (_c_int, [ctypes.POINTER(_vp), ctypes.c_size_t]),
     "hdrnet_host_ctx_destroy": (_c_int, [_vp]),
     "hdrnet_slice_apply_host_f32": (_c_int, [_vp] * 5 + [_c_int] * 9),
@@ -81,6 +83,13 @@ SIGNATURES = {
 
 # pixel storage formats (include/hdrnet_b200.h HDRNET_PX_*)
 PX_F32, PX_U8, PX_U16 = 0, 1, 2
+
+
+class TrainSample(ctypes.Structure):
+    """hdrnet_train_sample: one sample's descriptor for hdrnet_train_batch_f32."""
+    _fields_ = [("input", _vp), ("target", _vp), ("input_fmt", _c_int), ("target_fmt", _c_int),
+                ("H", _c_int), ("W", _c_int), ("fliplr", _c_int), ("flipud", _c_int),
+                ("rot90", _c_int), ("crop_y", _c_int), ("crop_x", _c_int)]
 
 _lock = threading.Lock()
 _lib = None

@@ -1,0 +1,324 @@
+#!/usr/bin/env python
+"""Training CLI: counterpart of the reference's ``hdrnet/bin/train.py`` with the same positional
+arguments, flags and defaults (train.py:188-244):
+
+    python -m hdrnet_b200.bin.train <checkpoint_dir> <data_dir> [--eval_data_dir DIR]
+        [--learning_rate 1e-4] [--batch_size 16] [--[no]fliplr|flipud|rotate|random_crop]
+        [--model_name HDRNetCurves] [--net_input_size 256] [--output_resolution 512 512] ...
+        [--max_steps N] [--seed S]
+
+``data_dir`` holds ``filelist.txt`` and the ``input/`` and ``output/`` folders (or is that
+``filelist.txt``); hdrnet_b200/data_pipeline.py keeps the decoded pairs on the device and builds
+each batch in one kernel.  Each step runs ``inference`` with the coefficient-network variables
+requiring grad, ``metrics.l2_loss`` and the per-image-mean ``metrics.psnr``, the backward and
+``torch.optim.Adam(learning_rate)``.  An exponential moving average (0.99, zero-debiased as TF's
+averages of tensors are) of loss and PSNR is logged every ``--log_interval`` seconds, and the
+scalars go to ``checkpoint_dir/train_log.jsonl``.
+
+Checkpoints (``model.ckpt-<step>`` every ``--checkpoint_interval`` seconds, ``on_stop.ckpt`` when
+the run stops, as train.py:181) are TF V2 bundles written by ``checkpoint.write_tf_checkpoint``:
+every ``inference/*`` variable (guide included), Adam's moments under TF's slot names
+``<var>/Adam`` and ``<var>/Adam_1``, ``beta1_power`` / ``beta2_power`` and ``global_step``, with
+``params.json`` beside them, so ``python -m hdrnet_b200.bin.run <checkpoint_dir> ...`` reads the
+directory as it is.  A ``checkpoint_dir`` that already holds a checkpoint is resumed: variables,
+moments and step are restored, and the batches continue where they would have (the sampler is a
+function of ``(seed, step)``).
+
+What is trained: the coefficient network.  The guide's backward, training-mode batch norm and the
+pyramid's resize VJP are not implemented, so ``--batch_norm`` and ``HDRNetGaussianPyrNN`` are
+refused before any data is read, with the models' own ``NotImplementedError``, and the guide
+variables are held fixed at their initial (or restored) values.
+
+Deliberate differences from the reference:
+
+* ``--max_steps`` (the reference runs until interrupted) and ``--seed`` are added;
+  ``--data_pipeline`` takes only ``ImageFilesDataPipeline`` (the tfrecord pipelines need TF);
+  ``--profiling`` is accepted and ignored.
+* The evaluation reads ``--eval_data_dir``.  The reference builds the eval pipeline but then
+  evaluates the training samples (train.py:86 takes ``train_data_pipeline.samples``, and :105
+  scores the training ``prediction``); that is not copied.
+* The network input is ``--net_input_size``; the reference's pipeline hard-codes 256
+  (data_pipeline.py:166).  The two are equal at the default.
+* ``torch.optim.Adam`` adds eps to sqrt(v_hat), the bias-corrected second moment; TF1's
+  AdamOptimizer adds its epsilon (``eps-hat``) to sqrt(v) and folds the bias correction into the
+  step size.  With eps = 1e-8 the two differ only while sqrt(v) is of the order of eps.
+* No queue runners, summaries or TF event files: batches are built on the device when needed and
+  the scalars go to ``train_log.jsonl``.  The random streams are not TF's (data_pipeline.py).
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import logging
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+from hdrnet_b200 import checkpoint, data_pipeline, metrics, models
+
+logging.basicConfig(format="[%(process)d] %(levelname)s %(filename)s:%(lineno)s | %(message)s")
+log = logging.getLogger("train")
+log.setLevel(logging.INFO)
+
+COEFFS = "inference/coefficients/"
+GUIDE = "inference/guide/"
+EMA_DECAY = 0.99
+BETA1, BETA2 = 0.9, 0.999       # tf.train.AdamOptimizer's and torch.optim.Adam's defaults
+
+
+def build_parser() -> argparse.ArgumentParser:
+    """train.py:188-244, plus --max_steps and --seed."""
+    parser = argparse.ArgumentParser(description="Train an HDRNet model from image pairs.")
+    req_grp = parser.add_argument_group("required")
+    req_grp.add_argument("checkpoint_dir", default=None, help="directory to save checkpoints to.")
+    req_grp.add_argument("data_dir", default=None, help="directory with filelist.txt, input/ and output/ (or that filelist.txt).")
+    req_grp.add_argument("--eval_data_dir", default=None, type=str, help="directory with the validation data.")
+
+    train_grp = parser.add_argument_group("training")
+    train_grp.add_argument("--learning_rate", default=1e-4, type=float, help="learning rate for the stochastic gradient update.")
+    train_grp.add_argument("--log_interval", type=int, default=1, help="interval between log messages (in s).")
+    train_grp.add_argument("--summary_interval", type=int, default=120, help="interval between scalar records in train_log.jsonl (in s)")
+    train_grp.add_argument("--checkpoint_interval", type=int, default=600, help="interval between model checkpoints (in s)")
+    train_grp.add_argument("--eval_interval", type=int, default=3600, help="interval between evaluations (in s)")
+    train_grp.add_argument("--max_steps", type=int, default=None, help="stop when the global step reaches this (default: run until interrupted).")
+    train_grp.add_argument("--seed", type=int, default=0, help="seed of the initial variables and of the data sampler.")
+
+    debug_grp = parser.add_argument_group("debug and profiling")
+    debug_grp.add_argument("--profiling", dest="profiling", action="store_true", help="accepted for compatibility; ignored.")
+    debug_grp.add_argument("--noprofiling", dest="profiling", action="store_false")
+
+    data_grp = parser.add_argument_group("data pipeline")
+    data_grp.add_argument("--batch_size", default=16, type=int, help="size of a batch for each gradient update.")
+    data_grp.add_argument("--data_threads", default=2, type=int, help="number of threads that decode the images at start-up.")
+    data_grp.add_argument("--rotate", dest="rotate", action="store_true", help="rotate data augmentation.")
+    data_grp.add_argument("--norotate", dest="rotate", action="store_false")
+    data_grp.add_argument("--flipud", dest="flipud", action="store_true", help="flip up/down data augmentation.")
+    data_grp.add_argument("--noflipud", dest="flipud", action="store_false")
+    data_grp.add_argument("--fliplr", dest="fliplr", action="store_true", help="flip left/right data augmentation.")
+    data_grp.add_argument("--nofliplr", dest="fliplr", action="store_false")
+    data_grp.add_argument("--random_crop", dest="random_crop", action="store_true", help="random crop data augmentation.")
+    data_grp.add_argument("--norandom_crop", dest="random_crop", action="store_false")
+
+    model_grp = parser.add_argument_group("model_params")
+    model_grp.add_argument("--model_name", default=models.__all__[0], type=str, help="classname of the model to use.",
+                           choices=models.__all__[:3])
+    model_grp.add_argument("--data_pipeline", default="ImageFilesDataPipeline", help="classname of the data pipeline to use.",
+                           choices=data_pipeline.__all__)
+    model_grp.add_argument("--net_input_size", default=256, type=int, help="size of the network's lowres image input.")
+    model_grp.add_argument("--output_resolution", default=[512, 512], type=int, nargs=2, help="resolution of the output image.")
+    model_grp.add_argument("--batch_norm", dest="batch_norm", action="store_true", help="normalize batches. If False, uses the moving averages.")
+    model_grp.add_argument("--nobatch_norm", dest="batch_norm", action="store_false")
+    model_grp.add_argument("--channel_multiplier", default=1, type=int, help="Factor to control net throughput (number of intermediate channels).")
+    model_grp.add_argument("--guide_complexity", default=16, type=int, help="Control complexity of the guide network.")
+    model_grp.add_argument("--luma_bins", default=8, type=int, help="Number of BGU bins for the luminance.")
+    model_grp.add_argument("--spatial_bin", default=16, type=int, help="Size of the spatial BGU bins (pixels).")
+
+    parser.set_defaults(profiling=False, flipud=False, fliplr=False, rotate=False, random_crop=True, batch_norm=False)
+    parser.model_group = model_grp
+    return parser
+
+
+def model_params(parser, args) -> dict:
+    """The model_params group, as train.py:250-252 collects it (and params.json stores it)."""
+    return {a.dest: getattr(args, a.dest, None) for a in parser.model_group._group_actions}
+
+
+def refuse_untrainable(params) -> None:
+    """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model
+    and training-mode batch norm.  Asks the models themselves, on the CPU, with a stand-in variable
+    that requires grad (they refuse before any device work)."""
+    S = int(params["net_input_size"])
+    if params["model_name"] == "HDRNetGaussianPyrNN":
+        probe = {COEFFS + "splat/conv1/weights": torch.zeros(1, requires_grad=True)}
+        models.HDRNetGaussianPyrNN.inference(torch.zeros(1, S, S, 3), torch.zeros(1, 1, 1, 3),
+                                             dict(params, weights=probe))
+    if params["batch_norm"]:
+        probe = {f"{scope}/BatchNorm/beta": torch.zeros(1, requires_grad=True)
+                 for scope, use_bn, _ in models._coefficient_specs(params) if use_bn}
+        getattr(models, params["model_name"])._coefficients(torch.zeros(1, S, S, 3), dict(params, weights=probe))
+
+
+def slot_names(name):
+    """TF's names of Adam's first and second moment of variable ``name``."""
+    return name + "/Adam", name + "/Adam_1"
+
+
+def checkpoint_tensors(variables: dict, moments: dict, step: int, ema: dict) -> dict:
+    """What a checkpoint holds, as numpy arrays: the variables, Adam's moments ``{name: (m, v)}``
+    under TF's slot names, ``global_step`` (int64), TF's ``beta1_power`` / ``beta2_power``
+    accumulators (beta^(step + 1)) and the logged moving averages."""
+    t = {k: np.asarray(v) for k, v in variables.items()}
+    for k, (m, v) in moments.items():
+        sm, sv = slot_names(k)
+        t[sm], t[sv] = np.asarray(m, np.float32), np.asarray(v, np.float32)
+    t["global_step"] = np.array(step, np.int64)
+    t["beta1_power"] = np.array(BETA1 ** (step + 1), np.float32)
+    t["beta2_power"] = np.array(BETA2 ** (step + 1), np.float32)
+    for key, val in ema.items():
+        t[f"train/{key}_ema"] = np.array(val, np.float64)
+    return t
+
+
+def restored_state(saved: dict, variables, trained):
+    """(variables, moments, step, ema) of a checkpoint read by read_tf_checkpoint: ``variables``
+    names every variable the model needs, ``trained`` those with Adam moments."""
+    missing = [k for k in list(variables) + [s for k in trained for s in slot_names(k)] + ["global_step"]
+               if k not in saved]
+    if missing:
+        raise ValueError(f"the checkpoint lacks {missing[0]} ({len(missing)} missing): not a training checkpoint "
+                         "of this model")
+    values = {k: np.asarray(saved[k], np.float32) for k in variables}
+    moments = {k: tuple(np.asarray(saved[s], np.float32) for s in slot_names(k)) for k in trained}
+    ema = {key[len("train/"):-len("_ema")]: float(v) for key, v in saved.items()
+           if key.startswith("train/") and key.endswith("_ema")}
+    return values, moments, int(saved["global_step"]), ema
+
+
+class Trainer:
+    """The training state of one run: variables, Adam, the data pipelines, the step counter."""
+
+    def __init__(self, args, params):
+        self.args, self.params = args, params
+        os.makedirs(args.checkpoint_dir, exist_ok=True)
+        self.mdl = getattr(models, params["model_name"])
+        self.device = torch.device("cuda", torch.cuda.current_device())
+        init = models.init_weights(params, seed=args.seed, model_name=params["model_name"])
+        self.weights = {k: torch.from_numpy(v).to(self.device) for k, v in init.items()}
+        self.names = sorted(k for k in self.weights if k.startswith(COEFFS))
+        for k in self.names:
+            self.weights[k].requires_grad_(True)
+        self.opt = torch.optim.Adam([self.weights[k] for k in self.names], lr=args.learning_rate,
+                                    betas=(BETA1, BETA2))
+        self.step = 0
+        self.ema = {"loss": 0.0, "psnr": 0.0}
+        self._resume()
+        log.info("%s: training the %d coefficient-network variables; the guide variables (%s*) are held fixed "
+                 "at their %s values", params["model_name"], len(self.names), GUIDE,
+                 "restored" if self.step else "initial")
+        self.train_data = data_pipeline.ImageFilesDataPipeline(
+            args.data_dir, batch_size=args.batch_size, output_resolution=args.output_resolution, shuffle=True,
+            fliplr=args.fliplr, flipud=args.flipud, rotate=args.rotate, random_crop=args.random_crop,
+            params=params, nthreads=args.data_threads, seed=args.seed, device=self.device)
+        self.eval_data = None
+        if args.eval_data_dir is not None:
+            self.eval_data = data_pipeline.ImageFilesDataPipeline(
+                args.eval_data_dir, batch_size=1, output_resolution=args.output_resolution, shuffle=False,
+                params=params, nthreads=1, device=self.device)
+        self.p = dict(params, weights=self.weights)
+
+    # ---- checkpoints ---------------------------------------------------------------------------
+    def _resume(self):
+        prefix = checkpoint.latest_checkpoint(self.args.checkpoint_dir)
+        if prefix is None:
+            return
+        values, moments, step, ema = restored_state(checkpoint.read_tf_checkpoint(prefix), self.weights, self.names)
+        with torch.no_grad():
+            for k, v in self.weights.items():
+                v.copy_(torch.from_numpy(values[k]).reshape(v.shape))
+        for k in self.names:
+            var = self.weights[k]
+            m, v = (torch.from_numpy(a).reshape(var.shape).to(self.device) for a in moments[k])
+            self.opt.state[var] = {"step": torch.tensor(float(step)), "exp_avg": m, "exp_avg_sq": v}
+        self.step = step
+        self.ema.update(ema)
+        log.info("resumed %s at step %d", prefix, step)
+
+    def save(self, name=None):
+        """Write ``model.ckpt-<step>`` (or ``name``) and params.json; returns the prefix."""
+        prefix = os.path.join(self.args.checkpoint_dir, name or f"model.ckpt-{self.step}")
+        moments = {}
+        for k in self.names:
+            st = self.opt.state.get(self.weights[k])
+            zero = torch.zeros_like(self.weights[k])
+            moments[k] = (st["exp_avg"] if st else zero).cpu().numpy(), (st["exp_avg_sq"] if st else zero).cpu().numpy()
+        variables = {k: v.detach().cpu().numpy() for k, v in self.weights.items()}
+        checkpoint.write_tf_checkpoint(prefix, checkpoint_tensors(variables, moments, self.step, self.ema))
+        with open(os.path.join(self.args.checkpoint_dir, "params.json"), "w") as f:
+            json.dump(self.params, f)
+        log.info("saved %s", prefix)
+        return prefix
+
+    # ---- steps ---------------------------------------------------------------------------------
+    def train_step(self):
+        """One gradient step on batch ``self.step``; returns (loss, psnr) as device scalars."""
+        batch = self.train_data.batch(self.step)
+        self.opt.zero_grad(set_to_none=True)
+        pred = self.mdl.inference(batch["lowres_input"], batch["image_input"], self.p)
+        loss = metrics.l2_loss(batch["image_output"], pred)
+        with torch.no_grad():
+            psnr = metrics.psnr(batch["image_output"], pred)
+        loss.backward()
+        self.opt.step()
+        self.step += 1
+        return loss.detach(), psnr
+
+    def evaluate(self) -> float:
+        """Mean PSNR over the eval set (batch 1, no augmentation, centre crop)."""
+        total = 0.0
+        with torch.no_grad():
+            for i in range(self.eval_data.nsamples):
+                b = self.eval_data.batch(i)
+                total += float(metrics.psnr(b["image_output"],
+                                            self.mdl.inference(b["lowres_input"], b["image_input"], self.p)))
+        return total / self.eval_data.nsamples
+
+    def record(self, rec):
+        with open(os.path.join(self.args.checkpoint_dir, "train_log.jsonl"), "a") as f:
+            f.write(json.dumps(rec) + "\n")
+
+    def run(self):
+        a = self.args
+        t0 = time.time()
+        last_log = last_summary = last_ckpt = last_eval = t0
+        try:
+            while a.max_steps is None or self.step < a.max_steps:
+                loss_t, psnr_t = self.train_step()
+                loss, psnr = float(loss_t), float(psnr_t)
+                for key, val in (("loss", loss), ("psnr", psnr)):
+                    self.ema[key] = EMA_DECAY * self.ema[key] + (1.0 - EMA_DECAY) * val
+                debias = 1.0 - EMA_DECAY ** self.step
+                loss_ema, psnr_ema = self.ema["loss"] / debias, self.ema["psnr"] / debias
+                now = time.time()
+                if now - last_log >= a.log_interval:
+                    log.info("Step %d | loss = %.4f | psnr = %.1f dB", self.step, loss_ema, psnr_ema)
+                    last_log = now
+                if now - last_summary >= a.summary_interval:
+                    self.record({"step": self.step, "time": now - t0, "loss": loss, "psnr": psnr,
+                                 "loss_ema": loss_ema, "psnr_ema": psnr_ema,
+                                 "learning_rate": a.learning_rate, "batch_size": a.batch_size})
+                    last_summary = now
+                if self.eval_data is not None and now - last_eval >= a.eval_interval:
+                    log.info("Evaluating on %d images at step %d", self.eval_data.nsamples, self.step)
+                    p = self.evaluate()
+                    log.info("  Evaluation PSNR = %.1f dB", p)
+                    self.record({"step": self.step, "time": time.time() - t0, "eval_psnr": p})
+                    last_eval = time.time()
+                if now - last_ckpt >= a.checkpoint_interval:
+                    self.save()
+                    last_ckpt = time.time()
+        except KeyboardInterrupt:
+            log.info("interrupted at step %d", self.step)
+        log.info("Training complete, saving chkpt %s", os.path.join(a.checkpoint_dir, "on_stop.ckpt"))
+        return self.save("on_stop.ckpt")
+
+
+def main(argv=None):
+    parser = build_parser()
+    args = parser.parse_args(argv)
+    params = model_params(parser, args)
+    refuse_untrainable(params)                       # before any data is read
+    if args.profiling:
+        log.warning("--profiling is accepted for compatibility and ignored")
+    if not torch.cuda.is_available():
+        raise RuntimeError("training needs a CUDA device; hdrnet_b200 has no CPU path")
+    return Trainer(args, params).run()
+
+
+if __name__ == "__main__":
+    try:
+        main()
+    except NotImplementedError as e:
+        sys.exit(f"train.py: {e}")

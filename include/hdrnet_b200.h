@@ -410,6 +410,37 @@ HDRNET_API int hdrnet_lowres_nearest_f32(const void* image, int fmt, float* lowr
                                          int W, int SH, int SW, void* stream);
 
 /*
+ * One training batch from decoded image pairs resident on the device: the augmentation of the
+ * reference's ImageFilesDataPipeline (hdrnet/data_pipeline.py:126-171) as one gather per output
+ * pixel, no workspace.  Per sample, in this order: flip left-right, flip up-down, rot90(k)
+ * counter-clockwise (equal to np.rot90(m, k)), then the oh x ow crop at (crop_y, crop_x) of the
+ * ROTATED extent ([W, H] for odd k).  Writes
+ *   fullres_in, fullres_out [B, oh, ow, 3] float32   the crop of input / target
+ *   lowres_in               [B, S, S, 3]   float32   TF1 resize_images(NEAREST_NEIGHBOR) of the
+ *                                                    input crop: src = min(floor(dst * (float)oh / S),
+ *                                                    oh - 1) (same for x), no half-pixel offset
+ * Integer pixels are converted as tf.to_float(v) / 255 (resp. 65535) in IEEE float32, the same
+ * bits as the model path's conversion.  The batch is ragged: each sample has its own source extent
+ * and each image its own format.  `samples` is a HOST array of B descriptors, read before the call
+ * returns; the image pointers in it are device pointers.  Errors: HDRNET_E_NULL_POINTER for a NULL
+ * output, descriptor array or image; HDRNET_E_BAD_SHAPE for B < 0, oh / ow / S < 1, H or W <= 0,
+ * k outside 0..3 or a crop outside the rotated source; HDRNET_E_UNSUPPORTED for an unknown format.
+ */
+typedef struct hdrnet_train_sample {
+  const void* input;    /* [H, W, 3] in input_fmt (HDRNET_PX_*), device memory  */
+  const void* target;   /* [H, W, 3] in target_fmt, the same extent              */
+  int input_fmt, target_fmt;
+  int H, W;             /* source extent                                          */
+  int fliplr, flipud;   /* nonzero: flip                                          */
+  int rot90;            /* k in 0..3                                              */
+  int crop_y, crop_x;   /* crop origin on the rotated extent                      */
+} hdrnet_train_sample;
+
+HDRNET_API int hdrnet_train_batch_f32(const hdrnet_train_sample* samples, int B, float* fullres_in,
+                                      float* fullres_out, float* lowres_in, int oh, int ow, int S,
+                                      void* stream);
+
+/*
  * Host-buffer path (what a CPU-tensor caller of the reference op gets: TF copies feeds to
  * the GPU and fetches back, hdrnet/bin/run.py:185).  A context owns device staging buffers
  * and streams; the call splits the batch into row bands, and pipelines H2D copy -> kernel

@@ -834,19 +834,10 @@ static int device_sms() {
   return sms;
 }
 
-static int patch_mode() {   // HDRNET_CONV_PATCH: 0 off, 1 / 2 force 4 / 8 channels per CTA (A/B knob, read once)
-  static const int mode = [] {
-    const char* e = std::getenv("HDRNET_CONV_PATCH");
-    return e ? std::atoi(e) : -1;
-  }();
-  return mode;
-}
-
-// 4 or 8 output channels per CTA for `ctas1` CTAs of the 4-channel form (tools/time_conv_layers.py)
+// 4 or 8 output channels per CTA for `ctas1` CTAs of the 4-channel form (tools/time_conv_layers.py):
+// a second CTA on an SM doubles its staging time
 static bool patch_two_groups(long long ctas1, int Cout, int K, int sms) {
-  const int mode = patch_mode();
-  const bool two = mode == 2 || (mode < 0 && ctas1 > sms);   // a second CTA on an SM doubles its staging time
-  return two && Cout % 8 == 0 && patch_smem_bytes(K, 2) <= 200 * 1024;
+  return ctas1 > sms && Cout % 8 == 0 && patch_smem_bytes(K, 2) <= 200 * 1024;
 }
 
 static int conv_dispatch(const ConvArgs& a, bool pdl, cudaStream_t stream) {
@@ -870,11 +861,11 @@ static int conv_dispatch(const ConvArgs& a, bool pdl, cudaStream_t stream) {
   // The shared-memory patch form: one memory round trip instead of one per 4 input channels, for
   // batch 1-8 of every layer of the network (tools/time_conv_layers.py compares the forms); the
   // bound below caps its 9x-redundant staging traffic, it is not a measured crossover.
-  if (patch_mode() != 0 && patch_ok(a)) {
+  if (patch_ok(a)) {
     const long long tiles = (total_px + kPatchPx - 1) / kPatchPx;
     const long long ctas1 = tiles * (a.Cout / 4);
     const bool two = patch_two_groups(ctas1, a.Cout, a.k * a.k * a.Cin, sms);
-    if (patch_mode() > 0 || (two ? ctas1 / 2 : ctas1) <= 32LL * sms)
+    if ((two ? ctas1 / 2 : ctas1) <= 32LL * sms)
       return two ? launch_conv_patch<2>(a, nullptr, pdl, stream) : launch_conv_patch<1>(a, nullptr, pdl, stream);
   }
   return (big_ctas >= 2LL * sms) ? launch_conv<2, 8>(a, stream) : launch_conv<1, 4>(a, stream);
@@ -888,7 +879,7 @@ static int conv_dispatch_pair(const ConvArgs& a, const ConvArgs& b, bool pdl, cu
     const long long px = static_cast<long long>(c.B) * c.OH * c.OW;
     return ((px + 127) / 128) < 96 && patch_ok(c);
   };
-  if (patch_mode() != 0 && a.Cout == b.Cout && a.B > 0 && b.B > 0 && small(a) && small(b) &&
+  if (a.Cout == b.Cout && a.B > 0 && b.B > 0 && small(a) && small(b) &&
       patch_slices(a.k * a.k * a.Cin) == patch_slices(b.k * b.k * b.Cin) &&
       !std::getenv("HDRNET_CONV_TCGEN05")) {
     const auto tiles = [](const ConvArgs& c) {
@@ -927,11 +918,7 @@ int hdrnet_fc_f32(const float* in, const float* w, const float* bias, float* out
   int ksplit = 1;
   while (ksplit < 8 && I / (ksplit * 2) >= 64) ksplit *= 2;
   const int slice = (I + ksplit - 1) / ksplit;
-  static const bool allow = [] {   // read once per process
-    const char* env = std::getenv("HDRNET_FC_CLUSTER");
-    return !(env && env[0] == '0');
-  }();
-  if (allow && O % 4 == 0 && (reinterpret_cast<uintptr_t>(w) & 15u) == 0 && ksplit >= 2 &&
+  if (O % 4 == 0 && (reinterpret_cast<uintptr_t>(w) & 15u) == 0 && ksplit >= 2 &&
       slice <= kFcCMaxSlice) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((O + kFcCOut - 1) / kFcCOut, ksplit, (B + kFcBatch - 1) / kFcBatch);

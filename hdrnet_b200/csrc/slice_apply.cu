@@ -272,42 +272,60 @@ slice_rows_any_kernel(const AnyArgs a) {
   }
 }
 
-// false when the shape does not suit it (slab rows larger than a quarter SM's shared memory,
-// images too narrow to fill a CTA): the caller then runs slice_generic_kernel.
-template <bool kApply, int kGc, int kIn, int kOut>
-static bool launch_rows_any_t(const AnyArgs& a, int max_smem, int sms, cudaStream_t stream, int* rc) {
-  constexpr int kGcp = (kGc + 3) / 4 * 4;
+// Compile-time channel count of the any-shape row kernel for these counts (0: run-time counts).  The
+// common shapes get one: the 3 -> 3 affine op with and without offset (what the TMA kernels take, at
+// widths / alignments they do not; ops_test.py:345-365), the pyramid grid (hdrnet_ops_test.py:91-100),
+// and the un-fused slice of a 12-channel grid.
+static int rows_any_gc(const AnyArgs& a, bool apply) {
+  if (!apply) return a.gc == 12 ? 12 : 0;
+  if (a.n_in == 3 && a.n_out == 3 && (a.J == 4 || a.J == 3)) return 3 * a.J;
+  if (a.n_in == 3 && a.n_out == 9 && a.J == 4) return 36;
+  return 0;
+}
+
+static int rows_any_smem_cap(int max_smem) { return (max_smem + 1024) / 4 - 1024; }   // 4 CTAs per SM
+
+// Dynamic shared memory of the any-shape row kernel, or 0 where the shape does not suit it (slab rows
+// larger than a quarter SM's shared memory, images too narrow to fill a CTA): slice_generic_kernel
+// runs then.
+static size_t rows_any_smem(const AnyArgs& a, bool apply, int max_smem) {
+  const int gc = rows_any_gc(a, apply);
   const size_t raw = (static_cast<size_t>(a.row_floats) + 3) & ~static_cast<size_t>(3);
-  const size_t slab = kGc > 0 ? static_cast<size_t>(a.g.gw) * a.g.gd * kGcp : raw;
+  const size_t slab = gc > 0 ? static_cast<size_t>(a.g.gw) * a.g.gd * ((gc + 3) / 4 * 4) : raw;
   const size_t smem = (2 * raw + slab) * sizeof(float);
-  if (a.g.W < 64 || smem > static_cast<size_t>((max_smem + 1024) / 4 - 1024)) return false;
+  if (a.g.W < 64 || smem > static_cast<size_t>(rows_any_smem_cap(max_smem))) return 0;
+  return smem;
+}
+
+static int rows_any_ctas(const SliceGeom& g, int sms) {
+  return static_cast<int>(std::min<long long>(static_cast<long long>(g.B) * g.rows, static_cast<long long>(sms) * 4));
+}
+
+template <bool kApply, int kGc, int kIn, int kOut>
+static int launch_rows_any_t(const AnyArgs& a, int ctas, size_t smem, int max_smem, cudaStream_t stream) {
   auto kern = slice_rows_any_kernel<kApply, kGc, kIn, kOut>;
   static std::atomic<int> granted{0};   // sticky per-function attribute: only ever raise it
   if (granted.load(std::memory_order_relaxed) < static_cast<int>(smem)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (max_smem + 1024) / 4 - 1024);
-    if (e != cudaSuccess) { *rc = static_cast<int>(e); return true; }
-    granted.store((max_smem + 1024) / 4 - 1024, std::memory_order_relaxed);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_any_smem_cap(max_smem));
+    if (e != cudaSuccess) return static_cast<int>(e);
+    granted.store(rows_any_smem_cap(max_smem), std::memory_order_relaxed);
   }
-  const long long rows = static_cast<long long>(a.g.B) * a.g.rows;
-  const int ctas = static_cast<int>(std::min<long long>(rows, static_cast<long long>(sms) * 4));
   kern<<<ctas, kAnyThreads, smem, stream>>>(a);
-  *rc = static_cast<int>(cudaGetLastError());
-  return true;
+  return static_cast<int>(cudaGetLastError());
 }
 
-// The common shapes get compile-time channel counts: the 3 -> 3 affine op with and without offset
-// (what the TMA kernels take, at widths / alignments they do not; ops_test.py:345-365), and the
-// un-fused slice of a 12-channel grid.
+// smem: rows_any_smem, non-zero
 template <bool kApply>
-static bool launch_rows_any(const AnyArgs& a, int max_smem, int sms, cudaStream_t stream, int* rc) {
+static int launch_rows_any(const AnyArgs& a, int ctas, size_t smem, int max_smem, cudaStream_t stream) {
+  const int gc = rows_any_gc(a, kApply);
   if constexpr (kApply) {
-    if (a.n_in == 3 && a.n_out == 3 && a.J == 4) return launch_rows_any_t<true, 12, 3, 3>(a, max_smem, sms, stream, rc);
-    if (a.n_in == 3 && a.n_out == 3 && a.J == 3) return launch_rows_any_t<true, 9, 3, 3>(a, max_smem, sms, stream, rc);
-    if (a.n_in == 3 && a.n_out == 9 && a.J == 4) return launch_rows_any_t<true, 36, 3, 9>(a, max_smem, sms, stream, rc);   // pyramid grid, hdrnet_ops_test.py:91-100
-    return launch_rows_any_t<true, 0, 0, 0>(a, max_smem, sms, stream, rc);
+    if (gc == 12) return launch_rows_any_t<true, 12, 3, 3>(a, ctas, smem, max_smem, stream);
+    if (gc == 9) return launch_rows_any_t<true, 9, 3, 3>(a, ctas, smem, max_smem, stream);
+    if (gc == 36) return launch_rows_any_t<true, 36, 3, 9>(a, ctas, smem, max_smem, stream);
+    return launch_rows_any_t<true, 0, 0, 0>(a, ctas, smem, max_smem, stream);
   } else {
-    if (a.gc == 12) return launch_rows_any_t<false, 12, 0, 0>(a, max_smem, sms, stream, rc);
-    return launch_rows_any_t<false, 0, 0, 0>(a, max_smem, sms, stream, rc);
+    if (gc == 12) return launch_rows_any_t<false, 12, 0, 0>(a, ctas, smem, max_smem, stream);
+    return launch_rows_any_t<false, 0, 0, 0>(a, ctas, smem, max_smem, stream);
   }
 }
 
@@ -782,12 +800,13 @@ static int device_texture_alignment() {
 }
 
 
-// Returns false when the TMA kernel cannot run these shapes.
+// Returns false when the TMA kernel cannot run these shapes.  threads: the threads that process
+// pixels (a quad each per segment).
 // tex_mode: the texture-assisted form double-buffers whole slab rows in raw0 / raw1 and needs no
 // separate slab region (lets 32x32x16 grids keep two CTAs per SM).
-static bool make_tma_plan(const SliceGeom& g, int max_smem, int sms, TmaPlan* out,
-                          bool tex_mode = false, int threads = kTmaThreads, int in_fmt = kPxF32,
-                          int out_fmt = kPxF32, int occ_override = 0, int grid_rows = 0) {
+// grid_rows: grid rows staged next to the slab rows (the slab warp of the issuer-warp form).
+static bool make_tma_plan(const SliceGeom& g, int max_smem, int sms, TmaPlan* out, bool tex_mode,
+                          int threads, int in_fmt = kPxF32, int out_fmt = kPxF32, int grid_rows = 0) {
   // Bulk copies move 16-byte units: a row and every segment must start on one.  float32 pixels
   // need W % 4 == 0, uint16 W % 8 == 0, uint8 W % 16 == 0 (12 / 6 / 3 bytes per pixel).
   const int in_bpp = 3 * px_bytes_per_channel(in_fmt), out_bpp = 3 * px_bytes_per_channel(out_fmt);
@@ -807,33 +826,15 @@ static bool make_tma_plan(const SliceGeom& g, int max_smem, int sms, TmaPlan* ou
   p.stage_bytes = round_up((p.off_out ? p.off_out + p.seg_px * out_bpp : p.off_guide + p.seg_px * 4), 128);
   p.off_raw = 256;  // barriers: up to 2 * kMaxStages + 4 (warp-specialised form) = 160 bytes
   p.off_slab = p.off_raw + round_up(2 * p.row_floats * 4, 128);
-  // grid_rows: grid rows staged next to the slab rows (the slab warp of the issuer-warp form)
   p.off_grid = p.off_slab;
   p.off_stage = p.off_slab + (tex_mode ? grid_rows * round_up(p.row_floats * 4, 128) : round_up(p.row_floats * 4, 128));
   // Residency: two CTAs per SM with a 4-stage ring; shrink the ring before giving up residency.
-  const int want_occ = occ_override > 0 ? occ_override : 2;
-  const int per_cta_3 = (max_smem + 1024) / 3 - 1024;
   const int per_cta_2 = (max_smem + 1024) / 2 - 1024;  // ~113 KB when 227 KB opt-in
   int stages = 0, resident = 0;
-  if (want_occ == 3) {
-    for (int ns = 3; ns >= 2; --ns)
-      if (p.off_stage + ns * p.stage_bytes <= per_cta_3) { stages = ns; resident = 3; break; }
-  }
-  if (occ_override >= 3) {  // issuer-warp form with small CTAs: deepest ring that keeps the residency
-    stages = 0;
-    const int per_cta_n = (max_smem + 1024) / occ_override - 1024;
-    for (int ns = 4; ns >= 2; --ns)
-      if (p.off_stage + ns * p.stage_bytes <= per_cta_n) { stages = ns; resident = occ_override; break; }
-  }
-  const int max_ns = 4;
-  if (stages == 0) {
-    for (int ns = max_ns; ns >= 2; --ns)
-      if (p.off_stage + ns * p.stage_bytes <= per_cta_2) { stages = ns; resident = 2; break; }
-  }
-  if (stages == 0) {
-    for (int ns = 4; ns >= 2; --ns)
-      if (p.off_stage + ns * p.stage_bytes <= max_smem) { stages = ns; resident = 1; break; }
-  }
+  for (int ns = 4; ns >= 2 && stages == 0; --ns)
+    if (p.off_stage + ns * p.stage_bytes <= per_cta_2) { stages = ns; resident = 2; }
+  for (int ns = 4; ns >= 2 && stages == 0; --ns)
+    if (p.off_stage + ns * p.stage_bytes <= max_smem) { stages = ns; resident = 1; }
   if (stages == 0) return false;
   p.stages = stages;
   p.resident = resident;
@@ -892,8 +893,8 @@ static int launch_tma(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream, 
 // whole workspace, not the part a call uses, so one entry serves every shape.  An entry remembers
 // an event recorded after the last launch that uses it; an evicted texture is destroyed only once
 // that event has completed (else it waits in a graveyard that later calls drain): a texture object
-// is never destroyed under a kernel that may still fetch through it.  This cache (and the tuning
-// record below) is the library's only process-wide state.
+// is never destroyed under a kernel that may still fetch through it.  This cache is the library's
+// only process-wide state.
 struct TexCacheEntry { const void* ptr; size_t bytes; int dev; cudaTextureObject_t tex; cudaEvent_t last_use; };
 constexpr int kTexCacheEntries = 16;
 static std::mutex g_tex_mutex;
@@ -966,11 +967,10 @@ struct GuideSpec {
 
 template <class GuideFn>
 static int launch_px_generic(const float* grid, const void* input, void* out, float* guide_out,
-                             const SliceGeom& g, long long npix, int sms, int in_fmt, int out_fmt,
+                             const SliceGeom& g, long long npix, int blocks, int in_fmt, int out_fmt,
                              const GuideFn& fn, cudaStream_t stream) {
   const unsigned char* in = static_cast<const unsigned char*>(input);
   unsigned char* o = static_cast<unsigned char*>(out);
-  const int blocks = generic_grid(npix, sms);
 #define HDRNET_PX_CASE(I, O)                                                                    \
   if (in_fmt == I && out_fmt == O) {                                                            \
     slice_apply_px_generic_kernel<GuideFn, I, O><<<blocks, 256, 0, stream>>>(grid, in, o,       \
@@ -986,24 +986,131 @@ static int launch_px_generic(const float* grid, const void* input, void* out, fl
   return HDRNET_E_UNSUPPORTED;
 }
 
-// Tuning record: read ONCE per process (first call) from the environment, for same-box A/B runs
-// (tools/ab_lib.py loads one copy of the library per setting).  Nothing reads the environment on
-// the launch path.
-//   HDRNET_ASYNC_THREADS = 512 | 352   CTA shape of the issuer-warp kernel (15 / 10 math warps)
-//   HDRNET_TEX_CHUNKS    = 4 | 5       corner chunks per pixel served by the texture pipe there
-//   HDRNET_FUSED_ASYNC   = 0 | 1       force the block-synchronous / issuer-warp fused-guide form
-//   HDRNET_ASYNC_SLAB    = 0 | 1       slab rows from the pre-pass / blended by a slab warp in the kernel
-struct Tuning { int async_threads, async_chunks, fused_async, async_slab; };
-static const Tuning& tuning() {
-  static const Tuning t = [] {
-    Tuning v{kAsyncThreadsDefault, kAsyncTexChunksDefault, -1, kAsyncSlabWarpDefault};
-    if (const char* e = std::getenv("HDRNET_ASYNC_SLAB")) v.async_slab = std::atoi(e) != 0 ? 1 : 0;
-    if (const char* e = std::getenv("HDRNET_ASYNC_THREADS")) { const int x = std::atoi(e); if (x == 512 || x == 352) v.async_threads = x; }
-    if (const char* e = std::getenv("HDRNET_TEX_CHUNKS")) { const int x = std::atoi(e); if (x == 4 || x == 5) v.async_chunks = x; }
-    if (const char* e = std::getenv("HDRNET_FUSED_ASYNC")) v.fused_async = std::atoi(e) != 0 ? 1 : 0;
-    return v;
-  }();
-  return t;
+// Which kernels one slice-apply call runs.  plan_slice_apply is the only place that decides it: the
+// launcher runs what it returns, and hdrnet_slice_apply_plan_ws reports it.
+struct ApplyForm {
+  int variant;        // HDRNET_VARIANT_GENERIC, _TMA, _TEX or _TEX_ASYNC
+  TmaPlan p;          // the row kernels' plan
+  bool pre_pass;      // texture-assisted forms: yblend_rows_kernel writes the slab rows first ...
+  bool slab_warp;     // ... or (issuer-warp form) a slab warp inside the kernel blends them
+  bool lean;          // issuer-warp form: index arithmetic per quad (x cells at least 4 pixels wide)
+  bool fused_async;   // texture-assisted, fused curves guide: the issuer-warp form
+  bool rows_any;      // GENERIC: the any-shape row kernel, else one thread per pixel
+  int ctas, threads;  // launch of the main kernel
+  size_t smem_bytes;
+};
+
+// g, n_in / n_out / has_offset, the guide mode and pixel formats of GuideSpec; aligned: every buffer
+// the call passes is 16-byte aligned; ws_base / ws_bytes: address and size of the lent workspace (0
+// without one).  HDRNET_E_UNSUPPORTED when a forced variant cannot run the call, or a float32
+// fused-guide call has no row-kernel form (the caller then runs the guide kernel first).
+static int plan_slice_apply(const SliceGeom& g, int n_in, int n_out, int has_offset, int mode, int in_fmt,
+                            int out_fmt, bool aligned, uintptr_t ws_base, size_t ws_bytes, int variant,
+                            ApplyForm* f) {
+  const int sms = device_sm_count();
+  const int max_smem = device_max_smem_optin();
+  const bool px = in_fmt != kPxF32 || out_fmt != kPxF32;
+  const long long npix = static_cast<long long>(g.B) * g.rows * g.W;
+  *f = ApplyForm{};
+
+  // The persistent row kernels take the 3 -> 3 affine op with offset on 16-byte aligned, bulk-copy
+  // sized rows, with (u8 | u16) -> u8 or f32 -> f32 pixels; everything else runs a generic kernel.
+  TmaPlan plan;
+  const bool row_shape = n_in == 3 && n_out == 3 && has_offset && aligned &&
+                         (!px || (in_fmt != kPxF32 && out_fmt == kPxU8)) &&
+                         make_tma_plan(g, max_smem, sms, &plan, false, kTmaThreads, in_fmt, out_fmt);
+  // Texture-assisted forms: possible when the caller lent a workspace for the slab rows, at the
+  // texture alignment.
+  const bool tex_ok = row_shape && ws_base != 0 && ws_base % device_texture_alignment() == 0 &&
+                      ws_bytes >= static_cast<size_t>(g.B) * g.rows * plan.row_floats * sizeof(float) &&
+                      ws_bytes / 16 <= (1u << 27);
+  // Issuer-warp form: float32 pixels, guide as an input, two CTAs per SM.
+  TmaPlan aplan, splan;
+  const bool async_ok = tex_ok && mode == 0 && !px &&
+                        make_tma_plan(g, max_smem, sms, &aplan, true, kAsyncThreads - 32) &&
+                        aplan.resident == 2 && aplan.seg_px <= aplan.threads * 4;
+  // ... with a SLAB WARP that blends each row's slab inside the kernel (no pre-pass launch): needs
+  // two more grid rows of shared memory next to the two slab rows, and still a ring of >= 3 stages,
+  // and workspace rows that are whole 128-byte cache lines (row bytes and base): a CTA fetches a
+  // workspace row through the texture path only after its own slab warp wrote it in THIS launch, and
+  // the caches start a launch invalid -- but a line shared by rows r and r + 1 would be cached,
+  // with row r + 1's bytes of the previous call, when row r is fetched (seen: 252-float rows)
+  const bool slab_lines = (static_cast<size_t>(plan.row_floats) * sizeof(float)) % 128 == 0 && ws_base % 128 == 0;
+  const bool slab_warp = async_ok && slab_lines &&
+                         make_tma_plan(g, max_smem, sms, &splan, true, kAsyncThreads - 32, kPxF32, kPxF32, 2) &&
+                         splan.resident == 2 && splan.seg_px <= splan.threads * 4 &&
+                         splan.stages >= kAsyncAutoMinStages;
+
+  const bool auto_req = variant == HDRNET_VARIANT_AUTO;
+  if (auto_req) {
+    // the texture-assisted forms pay a pre-pass launch or a slab warp: large images only
+    if (tex_ok && g.W >= 128 && npix >= (1LL << 21))
+      variant = (async_ok && aplan.stages >= kAsyncAutoMinStages) ? HDRNET_VARIANT_TEX_ASYNC : HDRNET_VARIANT_TEX;
+    else
+      variant = (row_shape && g.W >= 128) ? HDRNET_VARIANT_TMA : HDRNET_VARIANT_GENERIC;
+  }
+  f->variant = variant;
+
+  if (variant == HDRNET_VARIANT_GENERIC) {
+    // The float32 fused-guide forms exist only in the row kernels (the caller runs the standalone
+    // guide kernel first: see hdrnet_slice_apply_{curves,nn}_f32); integer pixels have a per-pixel
+    // fused kernel.  GENERIC on request is the one-thread-per-pixel L2 gather; AUTO takes the
+    // any-shape row kernel where it fits.
+    if (mode != 0 && !px) return HDRNET_E_UNSUPPORTED;
+    const int J = n_in + (has_offset ? 1 : 0);
+    const AnyArgs aa{nullptr, nullptr, nullptr, nullptr, g, n_in, n_out, J, n_out * J, g.gw * g.gd * n_out * J};
+    const size_t smem = (auto_req && mode == 0) ? rows_any_smem(aa, true, max_smem) : 0;
+    f->rows_any = smem != 0;
+    f->ctas = f->rows_any ? rows_any_ctas(g, sms) : generic_grid(npix, sms);
+    f->threads = f->rows_any ? kAnyThreads : 256;
+    f->smem_bytes = smem;
+    return HDRNET_OK;
+  }
+  if (variant == HDRNET_VARIANT_TMA) {
+    if (!row_shape) return HDRNET_E_UNSUPPORTED;
+    f->p = plan;
+  } else if (variant == HDRNET_VARIANT_TEX_ASYNC) {
+    if (!async_ok) return HDRNET_E_UNSUPPORTED;
+    f->slab_warp = slab_warp;
+    f->pre_pass = !slab_warp;
+    f->lean = static_cast<long long>(g.W) >= 4LL * g.gw;
+    f->p = slab_warp ? splan : aplan;
+  } else {   // HDRNET_VARIANT_TEX
+    if (!tex_ok) return HDRNET_E_UNSUPPORTED;
+    f->pre_pass = true;
+    // the fused-guide issuer-warp form (8 math warps + the issuer), for the curves guide only: for
+    // the pointwise-NN guide the block-synchronous form was as fast
+    TmaPlan fplan;
+    f->fused_async = mode == 1 &&
+                     make_tma_plan(g, max_smem, sms, &fplan, true, kFusedAsyncMathThreads, in_fmt, out_fmt) &&
+                     fplan.resident == kFusedAsyncResident && fplan.stages >= 3;
+    if (f->fused_async) {
+      f->p = fplan;
+    } else if (!make_tma_plan(g, max_smem, sms, &f->p, true, mode != 0 ? kTmaThreads : kTexThreads, in_fmt, out_fmt)) {
+      f->p = plan;   // the block-synchronous texture form: 512 threads for the op API, 256 for fused guides
+    }
+  }
+  // launch threads: the issuer-warp forms add the issuer warp, and the slab warp where there is one
+  const bool issuer = variant == HDRNET_VARIANT_TEX_ASYNC || f->fused_async;
+  f->ctas = f->p.ctas;
+  f->threads = f->p.threads + (issuer ? 32 : 0) + (f->slab_warp ? 32 : 0);
+  f->smem_bytes = f->p.smem_bytes;
+  return HDRNET_OK;
+}
+
+// The block-synchronous row kernel for the call's guide source (kTexChunks > 0: texture-assisted).
+template <int kTexChunks>
+static int launch_block_sync(const TmaArgs& a, const GuideSpec& gs, cudaStream_t stream) {
+  if (gs.mode == 1) { GuideCurves fn; fn.p = *gs.curves; return launch_tma<GuideCurves, kTexChunks>(a, fn, stream, gs.in_fmt, gs.out_fmt); }
+  if (gs.mode == 2 && gs.nn->feats <= 16) {
+    GuideNN<16> fn; fn.p = *gs.nn;
+    return launch_tma<GuideNN<16>, kTexChunks>(a, fn, stream, gs.in_fmt, gs.out_fmt);
+  }
+  if (gs.mode == 2) {
+    GuideNN<kMaxGuideFeats> fn; fn.p = *gs.nn;
+    return launch_tma<GuideNN<kMaxGuideFeats>, kTexChunks>(a, fn, stream, gs.in_fmt, gs.out_fmt);
+  }
+  return launch_tma<GuideFromInput, kTexChunks>(a, GuideFromInput{}, stream);
 }
 
 static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const void* input_v,
@@ -1032,146 +1139,56 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
     return HDRNET_E_UNSUPPORTED;
 
   const SliceGeom g = make_geom(B, H, W, rows, y_off, gh, gw, gd);
-  const int sms = device_sm_count();
-  const int max_smem = device_max_smem_optin();
-  const Tuning& tune = tuning();
+  const bool aligned = aligned16(grid) && aligned16(input) && aligned16(out) &&
+                       (gs.mode != 0 || aligned16(gs.guide)) && (gs.guide_out == nullptr || aligned16(gs.guide_out));
+  ApplyForm f;
+  rc = plan_slice_apply(g, n_in, n_out, has_offset, gs.mode, gs.in_fmt, gs.out_fmt, aligned,
+                        reinterpret_cast<uintptr_t>(gs.workspace), gs.workspace_bytes, variant, &f);
+  if (rc != HDRNET_OK) return rc;
 
-  // The persistent row kernels take the 3 -> 3 affine op with offset on 16-byte aligned, bulk-copy
-  // sized rows; everything else runs the generic kernel.
-  TmaPlan plan;
-  const bool row_shape = (n_in == 3 && n_out == 3 && has_offset) &&
-                         make_tma_plan(g, max_smem, sms, &plan, false,
-                                       gs.mode != 0 ? kFusedThreadsDefault : kTmaThreadsDefault, gs.in_fmt,
-                                       gs.out_fmt) &&
-                         // (u8 | u16) -> u8 and f32 -> f32 pixel forms
-                         (!px || (gs.in_fmt != kPxF32 && gs.out_fmt == kPxU8)) &&
-                         aligned16(grid) && aligned16(input) && aligned16(out) &&
-                         (gs.mode != 0 || aligned16(gs.guide)) &&
-                         (gs.guide_out == nullptr || aligned16(gs.guide_out));
-  // Texture-assisted forms: possible when the caller lent a workspace for the slab rows.
-  const size_t tex_need = row_shape ? static_cast<size_t>(B) * rows * plan.row_floats * sizeof(float) : 0;
-  const bool tex_ok = row_shape && gs.workspace && gs.workspace_bytes >= tex_need &&
-                      reinterpret_cast<uintptr_t>(gs.workspace) % device_texture_alignment() == 0 &&
-                      gs.workspace_bytes / 16 <= (1u << 27);
-  // Issuer-warp form: float32 pixels, guide as an input, a ring of >= 3 stages at two CTAs per SM.
-  TmaPlan aplan;
-  bool async_ok = tex_ok && gs.mode == 0 && !px &&
-                  make_tma_plan(g, max_smem, sms, &aplan, /*tex_mode=*/true, tune.async_threads - 32,
-                                kPxF32, kPxF32, 2) &&
-                  aplan.resident == 2 && aplan.seg_px <= aplan.threads * 4;
-  // ... with a SLAB WARP that blends each row's slab inside the kernel (no pre-pass launch): needs
-  // two more grid rows of shared memory next to the two slab rows, and still a ring of >= 3 stages
-  TmaPlan splan;
-  // ... and workspace rows that are whole 128-byte cache lines (row bytes and base): a CTA fetches a
-  // workspace row through the texture path only after its own slab warp wrote it in THIS launch, and
-  // the caches start a launch invalid -- but a line shared by rows r and r + 1 would be cached,
-  // with row r + 1's bytes of the previous call, when row r is fetched (seen: 252-float rows)
-  const bool slab_lines = (static_cast<size_t>(plan.row_floats) * sizeof(float)) % 128 == 0 &&
-                          (reinterpret_cast<uintptr_t>(gs.workspace) & 127u) == 0;
-  const bool slab_warp = async_ok && tune.async_slab && tune.async_threads == 352 && slab_lines &&
-                         make_tma_plan(g, max_smem, sms, &splan, /*tex_mode=*/true, tune.async_threads - 32,
-                                       kPxF32, kPxF32, 2, /*grid_rows=*/2) &&
-                         splan.resident == 2 && splan.seg_px <= splan.threads * 4 && splan.stages >= kAsyncAutoMinStages;
-  if (slab_warp) aplan = splan;
-  // ... and its fused-guide forms (8 math warps + the issuer).  AUTO takes it for the curves guide
-  // only: for the pointwise-NN guide the block-synchronous form was as fast.
-  TmaPlan fplan;
-  const bool fused_async_ok = tex_ok && gs.mode != 0 &&
-                              make_tma_plan(g, max_smem, sms, &fplan, /*tex_mode=*/true, kFusedAsyncMathThreads,
-                                            gs.in_fmt, gs.out_fmt, kFusedAsyncResident) &&
-                              fplan.resident == kFusedAsyncResident && fplan.stages >= 3;
-
-  const bool auto_generic = variant == HDRNET_VARIANT_AUTO;   // GENERIC on request = the one-thread-per-pixel L2 gather
-  if (variant == HDRNET_VARIANT_AUTO) {
-    // the texture-assisted forms pay a pre-pass launch: large images only
-    if (tex_ok && W >= 128 && npix >= (1LL << 21))
-      variant = (async_ok && aplan.stages >= kAsyncAutoMinStages) ? HDRNET_VARIANT_TEX_ASYNC : HDRNET_VARIANT_TEX;
-    else
-      variant = (row_shape && W >= 128) ? HDRNET_VARIANT_TMA : HDRNET_VARIANT_GENERIC;
+  if (f.variant == HDRNET_VARIANT_GENERIC) {
+    if (px) {   // integer pixel I/O on shapes the row kernel cannot take: the per-pixel fused kernel
+      if (gs.mode == 1) { GuideCurves fn; fn.p = *gs.curves;
+                          return launch_px_generic(grid, input_v, out_v, gs.guide_out, g, npix, f.ctas, gs.in_fmt, gs.out_fmt, fn, stream); }
+      if (gs.nn->feats <= 16) { GuideNN<16> fn; fn.p = *gs.nn;
+                                return launch_px_generic(grid, input_v, out_v, gs.guide_out, g, npix, f.ctas, gs.in_fmt, gs.out_fmt, fn, stream); }
+      GuideNN<kMaxGuideFeats> fn; fn.p = *gs.nn;
+      return launch_px_generic(grid, input_v, out_v, gs.guide_out, g, npix, f.ctas, gs.in_fmt, gs.out_fmt, fn, stream);
+    }
+    if (f.rows_any) {
+      const AnyArgs aa{grid, gs.guide, input, out, g, n_in, n_out, J, n_out * J, gw * gd * n_out * J};
+      return launch_rows_any<true>(aa, f.ctas, f.smem_bytes, device_max_smem_optin(), stream);
+    }
+    slice_generic_kernel<true><<<f.ctas, 256, 0, stream>>>(grid, gs.guide, input, out, g, n_in, n_out, J, npix);
+    return static_cast<int>(cudaGetLastError());
   }
 
-  if (variant == HDRNET_VARIANT_TEX || variant == HDRNET_VARIANT_TEX_ASYNC) {
-    if (!tex_ok) return HDRNET_E_UNSUPPORTED;
-    if (variant == HDRNET_VARIANT_TEX_ASYNC && !async_ok) return HDRNET_E_UNSUPPORTED;
-    TmaArgs a;
-    a.grid = grid; a.guide = gs.guide; a.guide_out = gs.guide_out;
-    a.input = static_cast<const unsigned char*>(input_v); a.out = static_cast<unsigned char*>(out_v);
-    a.g = g; a.yslab = gs.workspace;
-    cudaEvent_t tex_use = nullptr;
-    rc = get_slab_texture(gs.workspace, gs.workspace_bytes, &a.slab_tex, &tex_use);
+  TmaArgs a;
+  a.grid = grid; a.guide = gs.guide; a.guide_out = gs.guide_out;
+  a.input = static_cast<const unsigned char*>(input_v); a.out = static_cast<unsigned char*>(out_v);
+  a.g = g; a.p = f.p; a.slab_tex = 0; a.yslab = nullptr;
+  if (f.variant == HDRNET_VARIANT_TMA) return launch_block_sync<0>(a, gs, stream);
+
+  // texture-assisted forms
+  a.yslab = gs.workspace;
+  cudaEvent_t tex_use = nullptr;
+  rc = get_slab_texture(gs.workspace, gs.workspace_bytes, &a.slab_tex, &tex_use);
+  if (rc != 0) return rc;
+  if (f.pre_pass) {   // every row's y-pre-blended slab into the workspace
+    rc = launch_yblend(grid, gs.workspace, g, f.p.row_floats, stream);
     if (rc != 0) return rc;
-    const bool in_kernel_slab = variant == HDRNET_VARIANT_TEX_ASYNC && slab_warp;
-    if (!in_kernel_slab) {   // pre-pass: every row's y-pre-blended slab into the workspace
-      rc = launch_yblend(grid, gs.workspace, g, plan.row_floats, stream);
-      if (rc != 0) return rc;
-    }
-    if (variant == HDRNET_VARIANT_TEX_ASYNC) {
-      a.p = aplan;
-      a.guide_out = nullptr;
-      const bool lean = static_cast<long long>(W) >= 4LL * gw;   // x cells at least 4 pixels wide
-      rc = launch_async_form(a, tune.async_chunks, lean, tune.async_threads, in_kernel_slab, stream);
-    } else {
-      bool fused_async = gs.mode == 1;
-      if (tune.fused_async >= 0) fused_async = tune.fused_async != 0;
-      // the block-synchronous texture form: 512 threads for the op-API shape, 256 for fused guides
-      TmaPlan tplan;
-      if (!make_tma_plan(g, max_smem, sms, &tplan, /*tex_mode=*/true,
-                         gs.mode != 0 ? kFusedThreadsDefault : kTexThreadsDefault, gs.in_fmt, gs.out_fmt))
-        tplan = plan;
-      a.p = tplan;
-      if (gs.mode != 0 && fused_async && fused_async_ok) {
-        a.p = fplan;
-        rc = launch_async_fused(a, gs.mode, gs.curves, gs.nn, gs.in_fmt, gs.out_fmt, stream);
-      } else if (gs.mode == 1) {
-        GuideCurves fn; fn.p = *gs.curves;
-        rc = launch_tma<GuideCurves, kTexChunksDefault>(a, fn, stream, gs.in_fmt, gs.out_fmt);
-      } else if (gs.mode == 2 && gs.nn->feats <= 16) {
-        GuideNN<16> fn; fn.p = *gs.nn;
-        rc = launch_tma<GuideNN<16>, kTexChunksDefault>(a, fn, stream, gs.in_fmt, gs.out_fmt);
-      } else if (gs.mode == 2) {
-        GuideNN<kMaxGuideFeats> fn; fn.p = *gs.nn;
-        rc = launch_tma<GuideNN<kMaxGuideFeats>, kTexChunksDefault>(a, fn, stream, gs.in_fmt, gs.out_fmt);
-      } else {
-        rc = launch_tma<GuideFromInput, kTexChunksDefault>(a, GuideFromInput{}, stream);
-      }
-    }
-    // the texture must outlive every kernel that fetches through it (get_slab_texture)
-    if (rc == 0 && cudaEventRecord(tex_use, stream) != cudaSuccess) rc = static_cast<int>(cudaGetLastError());
-    return rc;
   }
-
-  if (variant == HDRNET_VARIANT_TMA) {
-    if (!row_shape) return HDRNET_E_UNSUPPORTED;
-    TmaArgs a;
-    a.grid = grid; a.guide = gs.guide; a.guide_out = gs.guide_out;
-    a.input = static_cast<const unsigned char*>(input_v); a.out = static_cast<unsigned char*>(out_v);
-    a.g = g; a.p = plan; a.slab_tex = 0; a.yslab = nullptr;
-    if (gs.mode == 0) return launch_tma(a, GuideFromInput{}, stream);
-    if (gs.mode == 1) { GuideCurves fn; fn.p = *gs.curves; return launch_tma(a, fn, stream, gs.in_fmt, gs.out_fmt); }
-    if (gs.nn->feats <= 16) { GuideNN<16> fn; fn.p = *gs.nn; return launch_tma(a, fn, stream, gs.in_fmt, gs.out_fmt); }
-    GuideNN<kMaxGuideFeats> fn; fn.p = *gs.nn;
-    return launch_tma(a, fn, stream, gs.in_fmt, gs.out_fmt);
+  if (f.variant == HDRNET_VARIANT_TEX_ASYNC) {
+    a.guide_out = nullptr;
+    rc = launch_async_form(a, f.lean, f.slab_warp, stream);
+  } else if (f.fused_async) {
+    rc = launch_async_fused(a, *gs.curves, gs.in_fmt, gs.out_fmt, stream);
+  } else {
+    rc = launch_block_sync<kSyncTexChunks>(a, gs, stream);
   }
-
-  // HDRNET_VARIANT_GENERIC: one thread per pixel.
-  if (px) {   // integer pixel I/O on shapes the row kernel cannot take: the per-pixel fused kernel
-    if (gs.mode == 1) { GuideCurves fn; fn.p = *gs.curves;
-                        return launch_px_generic(grid, input_v, out_v, gs.guide_out, g, npix, sms, gs.in_fmt, gs.out_fmt, fn, stream); }
-    if (gs.nn->feats <= 16) { GuideNN<16> fn; fn.p = *gs.nn;
-                              return launch_px_generic(grid, input_v, out_v, gs.guide_out, g, npix, sms, gs.in_fmt, gs.out_fmt, fn, stream); }
-    GuideNN<kMaxGuideFeats> fn; fn.p = *gs.nn;
-    return launch_px_generic(grid, input_v, out_v, gs.guide_out, g, npix, sms, gs.in_fmt, gs.out_fmt, fn, stream);
-  }
-  // The float32 fused-guide forms exist only in the row kernels; other shapes run the standalone
-  // guide kernel first (the caller does that: see hdrnet_slice_apply_{curves,nn}_f32).
-  if (gs.mode != 0) return HDRNET_E_UNSUPPORTED;
-  if (auto_generic) {   // AUTO on a shape the TMA kernels cannot take: the any-shape row kernel
-    AnyArgs aa{grid, gs.guide, input, out, g, n_in, n_out, J, n_out * J, gw * gd * n_out * J};
-    if (launch_rows_any<true>(aa, max_smem, sms, stream, &rc)) return rc;
-  }
-  slice_generic_kernel<true><<<generic_grid(npix, sms), 256, 0, stream>>>(
-      grid, gs.guide, input, out, g, n_in, n_out, J, npix);
-  return static_cast<int>(cudaGetLastError());
+  // the texture must outlive every kernel that fetches through it (get_slab_texture)
+  if (rc == 0 && cudaEventRecord(tex_use, stream) != cudaSuccess) rc = static_cast<int>(cudaGetLastError());
+  return rc;
 }
 
 // Internal launcher shared with the host path (host_path.cu): pixel buffers hold `rows`
@@ -1220,9 +1237,10 @@ int launch_slice(const float* grid, const float* guide, float* out, int B, int H
     slice_rows_tma_kernel<<<plan.ctas, kSliceThreads, plan.smem_bytes, stream>>>(a);
   } else {
     if (variant == HDRNET_VARIANT_AUTO) {
+      const int max_smem = device_max_smem_optin();
       AnyArgs aa{grid, guide, nullptr, out, g, 0, gc, 1, gc, gw * gd * gc};
-      int rc2 = 0;
-      if (launch_rows_any<false>(aa, device_max_smem_optin(), sms, stream, &rc2)) return rc2;
+      const size_t smem = rows_any_smem(aa, false, max_smem);
+      if (smem) return launch_rows_any<false>(aa, rows_any_ctas(g, sms), smem, max_smem, stream);
     }
     slice_generic_kernel<false><<<generic_grid(npix, sms), 256, 0, stream>>>(
         grid, guide, nullptr, out, g, 0, 0, gc, npix);
@@ -1440,37 +1458,18 @@ int hdrnet_slice_apply_plan_ws(int B, int H, int W, int gh, int gw, int gd, int 
                                int* threads, int* smem_bytes) {
   int rc = validate_common(B, H, W, gh, gw, gd);
   if (rc != HDRNET_OK) return rc;
-  const SliceGeom g = make_geom(B, H, W, H, 0, gh, gw, gd);
-  const int sms = device_sm_count();
-  const long long npix = static_cast<long long>(B) * H * W;
-  const bool tex = with_workspace && npix >= (1LL << 21);
-  TmaPlan plan;
-  const bool tma = (n_in == 3 && n_out == 3 && has_offset) && W >= 128 &&
-                   make_tma_plan(g, device_max_smem_optin(), sms, &plan, tex,
-                                 tex ? kTexThreadsDefault : kTmaThreadsDefault);
-  // what AUTO runs with a workspace: the issuer-warp form when its plan exists (see
-  // launch_slice_apply_impl); `threads` is the launch size (math warps + the issuer warp)
-  TmaPlan ap;
-  const bool async_form = tma && tex &&
-                          make_tma_plan(g, device_max_smem_optin(), sms, &ap, true, tuning().async_threads - 32,
-                                        kPxF32, kPxF32, 2) && ap.resident == 2 &&
-                          ap.seg_px <= ap.threads * 4 && ap.stages >= kAsyncAutoMinStages;
-  if (async_form) {
-    plan = ap;
-    plan.threads = tuning().async_threads;
-    TmaPlan sp;   // the slab-warp form (no pre-pass) when two more grid rows leave a ring of >= 3 stages
-    if (tuning().async_slab && tuning().async_threads == 352 && (static_cast<size_t>(gw) * gd * kGc * 4) % 128 == 0 &&
-        make_tma_plan(g, device_max_smem_optin(), sms, &sp, true, tuning().async_threads - 32, kPxF32, kPxF32, 2, 2) &&
-        sp.resident == 2 && sp.seg_px <= sp.threads * 4 && sp.stages >= kAsyncAutoMinStages) {
-      plan = sp;
-      plan.threads = tuning().async_threads + 32;
-    }
-  }
-  if (variant) *variant = tma ? (tex ? (async_form ? HDRNET_VARIANT_TEX_ASYNC : HDRNET_VARIANT_TEX) : HDRNET_VARIANT_TMA)
-                              : HDRNET_VARIANT_GENERIC;
-  if (ctas) *ctas = tma ? plan.ctas : generic_grid(npix, sms);
-  if (threads) *threads = tma ? plan.threads : 256;
-  if (smem_bytes) *smem_bytes = tma ? plan.smem_bytes : 0;
+  // the call described: AUTO, 16-byte aligned buffers and, with_workspace, a workspace of
+  // hdrnet_slice_apply_workspace_bytes at the device's texture alignment
+  ApplyForm f;
+  rc = plan_slice_apply(make_geom(B, H, W, H, 0, gh, gw, gd), n_in, n_out, has_offset, 0, kPxF32, kPxF32, true,
+                        with_workspace ? static_cast<uintptr_t>(device_texture_alignment()) : 0,
+                        with_workspace ? hdrnet_slice_apply_workspace_bytes(B, H, gw, gd) : 0,
+                        HDRNET_VARIANT_AUTO, &f);
+  if (rc != HDRNET_OK) return rc;
+  if (variant) *variant = f.variant;
+  if (ctas) *ctas = f.ctas;
+  if (threads) *threads = f.threads;
+  if (smem_bytes) *smem_bytes = static_cast<int>(f.smem_bytes);
   return HDRNET_OK;
 }
 

@@ -30,8 +30,7 @@ namespace hdrnet_b200 {
 //   * warp N-1 (one lane) is the ISSUER: it waits on done[s], issues the segment's ONE bulk store,
 //     refills the stage freed one item earlier, and after a row's last segment prefetches the slab
 //     row two rows ahead into the buffer that row just released.
-// 512 threads = 15 math warps (480 quads = one 1920-pixel segment, half a 4K row) + the issuer:
-// the 16th warp of the block-synchronous 512-thread form was idle at this width anyway.
+// 352 threads = 10 math warps (320 quads = one 1280-pixel segment, a third of a 4K row) + the issuer.
 //
 // kLean: index arithmetic per QUAD instead of per pixel where the x cells are at least 4 pixels
 // wide (W >= 4 gw).  floor(t_i) of the quad's pixels is floor(t_0) or floor(t_0) + 1 (t grows by
@@ -419,21 +418,26 @@ slice_apply_rows_async_kernel(const TmaArgs args) {
   }
 }
 
-template <int kTexChunks, bool kLean, int kThreads, bool kSlabWarp>
+template <bool kLean, bool kSlabWarp>
 static int launch_async(const TmaArgs& a, cudaStream_t stream) {
-  constexpr int kLaunchThreads = kThreads + (kSlabWarp ? 32 : 0);   // + the slab warp
-  auto kern = slice_apply_rows_async_kernel<kTexChunks, kLean, kLaunchThreads, 2, kSlabWarp>;
+  constexpr int kLaunchThreads = kAsyncThreads + (kSlabWarp ? 32 : 0);   // + the slab warp
+  auto kern = slice_apply_rows_async_kernel<kAsyncTexChunks, kLean, kLaunchThreads, 2, kSlabWarp>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, a.p.smem_bytes);
   if (e != cudaSuccess) return static_cast<int>(e);
   kern<<<a.p.ctas, kLaunchThreads, a.p.smem_bytes, stream>>>(a);
   return static_cast<int>(cudaGetLastError());
 }
 
+int launch_async_form(const TmaArgs& a, bool lean, bool slab_warp, cudaStream_t stream) {
+  if (slab_warp) return lean ? launch_async<true, true>(a, stream) : launch_async<false, true>(a, stream);
+  return lean ? launch_async<true, false>(a, stream) : launch_async<false, false>(a, stream);
+}
+
 // =========================================================================================
 // Issuer-warp control flow for the FUSED-GUIDE (model path) forms.
 // =========================================================================================
-// HDRNetCurves / HDRNetPointwiseNNGuide compute the guide from the pixel's RGB in registers
-// (24 B/px, models.py:43-59) and may read / write integer pixels.  This is the block-synchronous
+// HDRNetCurves computes the guide from the pixel's RGB in registers (24 B/px, models.py:43-59) and
+// may read / write integer pixels.  This is the block-synchronous
 // kernel's per-pixel code (slice_apply.cu, process_quad:
 // identical bits) under the issuer-warp control flow above: math warps that only wait for their
 // stage and ARRIVE on done[s], one warp that issues every bulk copy.  8 math warps + the issuer
@@ -555,52 +559,23 @@ slice_apply_rows_async_fused_kernel(const TmaArgs args, const __grid_constant__ 
   }
 }
 
-template <class GuideFn, int kIn, int kOut>
-static int launch_async_fused_fmt(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream) {
-  auto kern = slice_apply_rows_async_fused_kernel<GuideFn, kTexChunksDefault, kIn, kOut>;
+template <int kIn, int kOut>
+static int launch_async_fused_fmt(const TmaArgs& a, const GuideCurves& fn, cudaStream_t stream) {
+  auto kern = slice_apply_rows_async_fused_kernel<GuideCurves, kSyncTexChunks, kIn, kOut>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, a.p.smem_bytes);
   if (e != cudaSuccess) return static_cast<int>(e);
   kern<<<a.p.ctas, kFusedAsyncThreads, a.p.smem_bytes, stream>>>(a, fn);
   return static_cast<int>(cudaGetLastError());
 }
 
-template <class GuideFn>
-static int launch_async_fused_guide(const TmaArgs& a, const GuideFn& fn, int in_fmt, int out_fmt,
-                                    cudaStream_t stream) {
-  if (in_fmt == kPxF32 && out_fmt == kPxF32) return launch_async_fused_fmt<GuideFn, kPxF32, kPxF32>(a, fn, stream);
-  if (in_fmt == kPxU8 && out_fmt == kPxU8) return launch_async_fused_fmt<GuideFn, kPxU8, kPxU8>(a, fn, stream);
-  if (in_fmt == kPxU16 && out_fmt == kPxU8) return launch_async_fused_fmt<GuideFn, kPxU16, kPxU8>(a, fn, stream);
-  return HDRNET_E_UNSUPPORTED;
-}
-
-// mode 1 = curves guide, 2 = pointwise-NN guide (plan: (kFusedAsyncThreads - 32) quads per segment)
-int launch_async_fused(const TmaArgs& a, int mode, const CurvesGuideParams* curves, const NNGuideParams* nn,
-                       int in_fmt, int out_fmt, cudaStream_t stream) {
-  if (mode == 1) { GuideCurves fn; fn.p = *curves; return launch_async_fused_guide(a, fn, in_fmt, out_fmt, stream); }
-  if (mode == 2) {
-    if (nn->feats <= 16) { GuideNN<16> fn; fn.p = *nn; return launch_async_fused_guide(a, fn, in_fmt, out_fmt, stream); }
-    GuideNN<kMaxGuideFeats> fn; fn.p = *nn;
-    return launch_async_fused_guide(a, fn, in_fmt, out_fmt, stream);
-  }
-  return HDRNET_E_UNSUPPORTED;
-}
-
-// chunks (4 | 5), per-quad index arithmetic or not, CTA shape (512 | 352 threads: math warps + the
-// issuer), slab warp or pre-pass -> instantiation
-template <int kThreads, bool kSlabWarp>
-static int launch_async_shape(const TmaArgs& a, int chunks, bool lean, cudaStream_t stream) {
-  if (lean) return chunks == 4 ? launch_async<4, true, kThreads, kSlabWarp>(a, stream)
-                               : launch_async<5, true, kThreads, kSlabWarp>(a, stream);
-  return chunks == 4 ? launch_async<4, false, kThreads, kSlabWarp>(a, stream)
-                     : launch_async<5, false, kThreads, kSlabWarp>(a, stream);
-}
-
-int launch_async_form(const TmaArgs& a, int chunks, bool lean, int threads, bool slab_warp, cudaStream_t stream) {
-  if (threads == 352)
-    return slab_warp ? launch_async_shape<352, true>(a, chunks, lean, stream)
-                     : launch_async_shape<352, false>(a, chunks, lean, stream);
-  if (threads == 512)   // 15 math warps + issuer + slab warp would be 544 threads: pre-pass only
-    return slab_warp ? HDRNET_E_UNSUPPORTED : launch_async_shape<512, false>(a, chunks, lean, stream);
+// plan: (kFusedAsyncThreads - 32) quads per segment
+int launch_async_fused(const TmaArgs& a, const CurvesGuideParams& curves, int in_fmt, int out_fmt,
+                       cudaStream_t stream) {
+  GuideCurves fn;
+  fn.p = curves;
+  if (in_fmt == kPxF32 && out_fmt == kPxF32) return launch_async_fused_fmt<kPxF32, kPxF32>(a, fn, stream);
+  if (in_fmt == kPxU8 && out_fmt == kPxU8) return launch_async_fused_fmt<kPxU8, kPxU8>(a, fn, stream);
+  if (in_fmt == kPxU16 && out_fmt == kPxU8) return launch_async_fused_fmt<kPxU16, kPxU8>(a, fn, stream);
   return HDRNET_E_UNSUPPORTED;
 }
 

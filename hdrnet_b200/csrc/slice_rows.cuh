@@ -101,30 +101,29 @@ __device__ __forceinline__ float load_channel(const unsigned char* base, long lo
 // Persistent TMA row kernel: n_in = 3, n_out = 3, has_offset (gc = 12), W % 4 == 0.
 // =========================================================================================
 
-constexpr int kTmaThreads = 256;
-constexpr int kTmaThreadsDefault = 256;  // all-LSU form
-constexpr int kTexThreadsDefault = 512;  // block-synchronous texture-assisted form (64 registers)
-constexpr int kFusedThreadsDefault = 256; // fused-guide forms of the block-synchronous kernel
-constexpr int kAsyncThreadsDefault = 352; // issuer-warp form: 10 math warps + the issuer, two CTAs per SM, 88 registers
+constexpr int kTmaThreads = 256;    // all-LSU form, and every form of the block-synchronous kernel with a fused guide
+constexpr int kTexThreads = 512;    // block-synchronous texture-assisted form of the op API (64 registers)
+constexpr int kAsyncThreads = 352;  // issuer-warp form: 10 math warps + the issuer, two CTAs per SM, 88 registers
 // AUTO takes the issuer-warp form only with a ring of >= 3 stages at two CTAs per SM: with the two
 // stages that 32x32 grids leave (24 / 48 KB of slab rows) the block-synchronous form was faster.
 // Checked on an H100 (tools/ab_lib.py, 4K x 8, medians of interleaved bursts, 400 W card): at
-// 16x16x8 the default (352 + slab warp, 5 texture chunks) 0.805 ms against 0.827 without the slab
+// 16x16x8 the kept form (352 + slab warp, 5 texture chunks) 0.805 ms against 0.827 without the slab
 // warp, 0.838 with 4 texture chunks, 0.841 at 512 threads, 0.931 block-synchronous texture form,
 // 0.949 all-LSU; at 32x32x16 1.258 against 1.255 (4 chunks), 1.388 (512), 1.370 (block-synchronous).
+// The 4-chunk and 512-thread shapes of the issuer-warp form were removed on these numbers.
 constexpr int kAsyncAutoMinStages = 3;
-constexpr int kAsyncTexChunksDefault = 5; // corner chunks per pixel through the texture pipe (HDRNET_TEX_CHUNKS)
-constexpr int kAsyncSlabWarpDefault = 1;  // slab rows blended by a slab warp inside the kernel: no pre-pass (HDRNET_ASYNC_SLAB)
+constexpr int kAsyncTexChunks = 5;  // corner chunks per pixel through the texture pipe in the issuer-warp form
 constexpr int kMaxStages = 8;
-constexpr int kTexChunksDefault = 4;   // texture chunks of the block-synchronous and opt-in forms
+constexpr int kSyncTexChunks = 4;   // texture chunks of the block-synchronous forms (and of the fused-guide
+                                    // issuer-warp form, which runs their per-pixel code)
 constexpr int kGc = 12;
 
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
 struct TmaPlan {
   int ctas;
-  int threads;     // threads per CTA (256, or 512 = the 64-register / 32-warps-per-SM form)
-  int resident;    // CTAs per SM the plan was sized for (1, 2 or 3)
+  int threads;     // threads that process pixels (issuer-warp forms: the math warps)
+  int resident;    // CTAs per SM the plan was sized for (1 or 2)
   int stages;
   int nseg;        // segments per row
   int seg_px;      // pixels per segment (multiple of 4, <= 4 * kTmaThreads)
@@ -290,11 +289,12 @@ __device__ __forceinline__ void process_quad(const TmaArgs& args, const GuideFn&
 }
 
 // Entry points of slice_apply_async.cu (non-template: the arguments select the instantiation).
-int launch_async_form(const TmaArgs& a, int chunks, bool lean, int threads, bool slab_warp, cudaStream_t stream);
-int launch_async_fused(const TmaArgs& a, int mode, const CurvesGuideParams* curves, const NNGuideParams* nn,
-                       int in_fmt, int out_fmt, cudaStream_t stream);
-// fused-guide issuer-warp form: 8 math warps + the issuer warp, 2 CTAs per SM (96 registers); preferred
-// to 6 math warps x 3 CTAs and 10 x 2 (both 80 registers) for the curves guide.
+int launch_async_form(const TmaArgs& a, bool lean, bool slab_warp, cudaStream_t stream);
+int launch_async_fused(const TmaArgs& a, const CurvesGuideParams& curves, int in_fmt, int out_fmt,
+                       cudaStream_t stream);
+// fused-guide issuer-warp form (curves guide only: for the pointwise-NN guide the block-synchronous
+// form was as fast, and its issuer-warp form was removed): 8 math warps + the issuer warp, 2 CTAs per
+// SM (96 registers); preferred to 6 math warps x 3 CTAs and 10 x 2 (both 80 registers).
 constexpr int kFusedAsyncMathThreads = 256;
 constexpr int kFusedAsyncResident = 2;
 

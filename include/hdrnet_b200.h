@@ -169,13 +169,15 @@ HDRNET_API int hdrnet_slice_indices_i32(const float* guide, int32_t* idx, int B,
                              int gw, int gd, void* stream);
 
 /*
- * Kernel-introspection for benchmarks: which variant AUTO would pick for these shapes, and
- * the launch geometry of the TMA kernel (CTAs, threads, dynamic shared memory bytes).
+ * Kernel-introspection for benchmarks: the variant AUTO runs for these shapes with 16-byte aligned
+ * buffers, and the launch geometry of its main kernel (CTAs, threads, dynamic shared memory bytes).
+ * The same planner decides the launches, so the report is what the call runs.
  */
 HDRNET_API int hdrnet_slice_apply_plan(int B, int H, int W, int gh, int gw, int gd, int n_in, int n_out,
                             int has_offset, int* variant, int* ctas, int* threads,
                             int* smem_bytes);
-/* Same, for a call that lends a workspace (hdrnet_slice_apply_f32_ws). */
+/* Same, for a call that lends a workspace (hdrnet_slice_apply_f32_ws) of
+ * hdrnet_slice_apply_workspace_bytes at the device's texture alignment. */
 HDRNET_API int hdrnet_slice_apply_plan_ws(int B, int H, int W, int gh, int gw, int gd, int n_in,
                                           int n_out, int has_offset, int with_workspace,
                                           int* variant, int* ctas, int* threads, int* smem_bytes);

@@ -193,3 +193,6 @@ def test_kernel_selection_plan(built_lib):
     assert _plan(lib, 8, 2160, 3841, 16, 16, 8, 1)[0] == _lib.VARIANT_GENERIC
     assert _plan(lib, 8, 2160, 3840, 16, 16, 8, 1, n_out=4)[0] == _lib.VARIANT_GENERIC
     assert _plan(lib, 1, 16, 64, 4, 4, 4, 1)[0] == _lib.VARIANT_GENERIC
+    # 96 x 16 cells: two 72 KB grid rows leave no room for the all-LSU row kernel's slab and ring, so
+    # no row kernel (nor its texture-assisted forms) takes the call, workspace or not
+    assert _plan(lib, 2, 1080, 1920, 16, 96, 16, 1)[0] == _lib.VARIANT_GENERIC

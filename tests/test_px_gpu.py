@@ -10,14 +10,12 @@ What is checked, and to what bar:
     code value (and < 0.1 % of samples) when the float path runs a different family;
   * the whole image path against the oracle model: within one code value.
 """
-import os
-
 import numpy as np
 import pytest
 import torch
 
 import oracle
-from hdrnet_b200 import _lib, models
+from hdrnet_b200 import _lib, hdrnet_ops, models
 from hdrnet_b200.bin import run
 from oracle import model_np as M
 
@@ -170,22 +168,39 @@ def test_unsupported_formats_are_refused():
         models.lowres_from_image(torch.zeros(1, 4, 4, 3, dtype=torch.int32, device="cuda"), 2)
 
 
-# ---- fused-guide forms under the issuer-warp control flow ------------------------------------------
+# ---- fused-guide texture-assisted forms against the un-fused composition -------------------------
 def test_fused_guide_issuer_warp_form_is_bitwise_equal():
-    """HDRNET_FUSED_ASYNC=1 / 0 force the issuer-warp / the block-synchronous control flow around
-    the same per-pixel code (process_quad): the output of the model's full-resolution stage must
-    not change by a bit, for both guides and all three pixel formats (AUTO picks one form per guide
-    type).  One process per setting: the library reads its tuning record once."""
-    import subprocess, sys
-    runner = os.path.join(os.path.dirname(os.path.abspath(__file__)), "knob_runner.py")
-    shas = []
-    for flag in ("0", "1"):
-        env = {k: v for k, v in os.environ.items() if not k.startswith("HDRNET_")}
-        env["HDRNET_FUSED_ASYNC"] = flag
-        out = subprocess.run([sys.executable, runner, "fused"], env=env, capture_output=True, text=True, timeout=600)
-        assert out.returncode == 0, out.stdout + out.stderr
-        shas.append(dict(l.split()[1:3] for l in out.stdout.splitlines() if l.startswith("SHA256")))
-    assert len(shas[0]) == 6 and shas[0] == shas[1]
+    """At >= 2 Mi pixels the model's full-resolution stage runs the texture-assisted fused-guide forms:
+    the issuer-warp form for the curves guide, the block-synchronous one for the pointwise-NN guide.
+    For both guides and all three pixel formats they must give the bits of the un-fused composition:
+    the standalone guide kernel, then the op API's block-synchronous texture form
+    (HDRNET_VARIANT_TEX) on the float image; integer pixels are compared with that float result
+    quantised on the host."""
+    B, H, W = 2, 300, 3840
+    for kind in ("curves", "nn"):
+        cls = models.HDRNetCurves if kind == "curves" else models.HDRNetPointwiseNNGuide
+        p = params_for(kind)
+        for dtype in (np.float32, np.uint8, np.uint16):
+            rng = np.random.RandomState(5)
+            if dtype == np.float32:
+                im = rng.rand(B, H, W, 3).astype(np.float32)
+                im_f = im
+                low = cuda(rng.rand(B, 64, 64, 3).astype(np.float32))
+            else:
+                im = rand_image(rng, B, H, W, dtype)
+                im_f = np.stack([run.img_as_float(im[b]) for b in range(B)])
+                low = models.lowres_from_image(cuda(im), p["net_input_size"])
+            coeffs = cls._coefficients(low, p)
+            out_dtype = torch.float32 if dtype == np.float32 else torch.uint8
+            got = cls._fullres(coeffs, cuda(im), p, out_dtype).cpu().numpy()
+            f = cuda(im_f)
+            guide = cls._guide(f, p)
+            gh, gw, gd = coeffs.shape[1:4]
+            want = hdrnet_ops.bilateral_slice_apply(coeffs.reshape(B, gh, gw, gd, 12), guide, f, True,
+                                                    variant=_lib.VARIANT_TEX).cpu().numpy()
+            if dtype != np.float32:
+                want = quantize(want)
+            assert np.array_equal(got, want), f"{kind} guide, {np.dtype(dtype).name} pixels"
 
 
 @pytest.mark.parametrize("kind,dtype,pinned", [("curves", torch.uint8, True), ("nn", torch.uint16, True),

@@ -3,7 +3,8 @@ the oracle on the same seeded inputs, against the committed golden fixtures from
 reference's JAX file, and -- at BASELINE.json's full 4K size -- against the full oracle on
 one frame plus size-independent properties.  Tolerance: 1e-5 relative (tests/util.py);
 cell indices bit-exact."""
-import os
+import ctypes
+import re
 
 import numpy as np
 import pytest
@@ -212,36 +213,104 @@ def test_row_kernels_are_bitwise_equal():
         assert np.array_equal(a, run_apply(grid, gu, inp, True, "tex_async"))
 
 
-def _knob_shas(env, *args):
-    """{case: sha256} of the seeded cases of tests/knob_runner.py, computed in a process of its own
-    (the library reads its tuning record once per process)."""
-    import subprocess, sys
-    e = {k: v for k, v in os.environ.items() if not k.startswith("HDRNET_")}
-    e.update(env)
-    runner = os.path.join(os.path.dirname(os.path.abspath(__file__)), "knob_runner.py")
-    out = subprocess.run([sys.executable, runner, *map(str, args)], env=e, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stdout + out.stderr
-    return dict(l.split()[1:3] for l in out.stdout.splitlines() if l.startswith("SHA256"))
+def launched_kernels(fn, attempts=3):
+    """Names of the library's CUDA kernels fn() launches, from torch.profiler (demangled).  Now and
+    then a short profiling session comes back with no kernel record at all; a call always launches
+    at least one kernel, so such an empty capture is repeated."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(attempts):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+                 and "hdrnet_b200::" in e.name]
+        if names:
+            break
+    return names
 
 
-@pytest.mark.parametrize("env", [dict(HDRNET_ASYNC_THREADS="512"), dict(HDRNET_ASYNC_SLAB="0"),
-                                 dict(HDRNET_ASYNC_SLAB="1"), dict(HDRNET_ASYNC_SLAB="1", HDRNET_TEX_CHUNKS="4"),
-                                 dict(HDRNET_ASYNC_THREADS="512", HDRNET_TEX_CHUNKS="4")],
-                         ids=lambda e: ",".join(f"{k[7:].lower()}={v}" for k, v in e.items()))
-def test_issuer_warp_kernel_knobs_are_bitwise_equal(env):
-    """Both CTA shapes of the issuer-warp form, slab rows from the pre-pass or from the slab warp
-    inside the kernel, and 4 / 5 of a pixel's 12 corner chunks on the texture pipe: identical bits; also on narrow x cells (W < 4 gw: per-pixel indices), many rows
-    per CTA, a ragged last segment and out-of-range guides."""
-    import hashlib
-    import knob_runner
-    got = _knob_shas(env, "apply", _lib.VARIANT_TEX_ASYNC)
-    for k, (seed, B, H, W, gh, gw, gd, edge) in enumerate(knob_runner.APPLY_CASES):
-        grid, guide, inp = rand_case(seed, B, H, W, gh, gw, gd, signed=True)
-        if edge:
-            guide[0, :, ::5] = 1.75
-            guide[0, :, 1::5] = -0.6
-        want = hashlib.sha256(run_apply(grid, guide, inp, True, "tex").tobytes()).hexdigest()
-        assert got[f"apply{k}"] == want, (env, k)
+def _async_instantiation(names):
+    """(slab warp, lean) of the one issuer-warp kernel among `names`."""
+    got = [m.groups() for m in (re.search(r"slice_apply_rows_async_kernel<5, (true|false), (352|384), 2, (true|false)>", n)
+                                for n in names) if m]
+    assert len(got) == 1, names
+    lean, threads, slab = got[0]
+    assert (threads == "384") == (slab == "true"), got
+    return slab == "true", lean == "true"
+
+
+# (seed, B, H, W, gh, gw, gd, out-of-range guides) -> (slab warp, lean) of the issuer-warp kernel that runs
+ISSUER_WARP_CASES = {
+    (5, 2, 64, 3840, 16, 16, 8, False): (True, True),     # headline row shape
+    (6, 1, 700, 1028, 5, 7, 3, True): (False, True),      # many rows per CTA, ragged last segment, edge guides, 1008-byte slab rows
+    (7, 3, 9, 128, 8, 64, 4, False): (True, False),       # W < 4 gw: per-pixel indices
+    (8, 2, 300, 2048, 8, 8, 4, True): (True, True),       # small grid, 1536-byte slab rows, several rows per grid row
+    (9, 1, 40, 3840, 32, 32, 16, False): (False, True),   # no room for the slab warp's grid rows
+    (10, 2, 24, 128, 16, 63, 3, True): (False, False),    # per-pixel indices; 9072-byte slab rows are not whole lines
+}
+assert set(ISSUER_WARP_CASES.values()) == {(s, l) for s in (True, False) for l in (True, False)}
+
+
+@pytest.mark.parametrize("case", list(ISSUER_WARP_CASES), ids=lambda c: "x".join(map(str, c[1:7])))
+def test_issuer_warp_kernel_is_bitwise_the_block_synchronous_one(case):
+    """Every instantiation of the issuer-warp form (slab rows from the pre-pass or from the slab warp
+    inside the kernel; per-quad or per-pixel indices; which one runs is read from the profiler) gives
+    the bits of the block-synchronous texture form, also on many rows per CTA, a ragged last segment
+    and out-of-range guides.  The call comes right after one with another grid, which leaves its slab
+    rows in the workspace block the caching allocator hands to the next call: a kernel that read stale
+    rows (e.g. through a cache) would show it."""
+    seed, B, H, W, gh, gw, gd, edge = case
+    grid, guide, inp = rand_case(seed, B, H, W, gh, gw, gd, signed=True)
+    if edge:
+        guide[0, :, ::5] = 1.75
+        guide[0, :, 1::5] = -0.6
+    want = run_apply(grid, guide, inp, True, "tex")
+    g, u, i = cuda(grid), cuda(guide), cuda(inp)
+    other = cuda(grid[::-1, ::-1] * 1.5 + 0.25)
+    hdrnet_ops.bilateral_slice_apply(other, u, i, True, variant=_lib.VARIANT_TEX_ASYNC)
+    got = []
+    names = launched_kernels(lambda: got.append(
+        hdrnet_ops.bilateral_slice_apply(g, u, i, True, variant=_lib.VARIANT_TEX_ASYNC)))
+    slab_warp, lean = _async_instantiation(names)
+    assert (slab_warp, lean) == ISSUER_WARP_CASES[case], names
+    assert any("yblend_rows_kernel" in n for n in names) == (not slab_warp), names
+    assert np.array_equal(got[0].cpu().numpy(), want)
+
+
+def plan(B, H, W, gh, gw, gd, with_ws):
+    """(variant, threads, smem_bytes) hdrnet_slice_apply_plan_ws reports for AUTO."""
+    v, c, t, sm = (ctypes.c_int() for _ in range(4))
+    _lib.check(_lib.load().hdrnet_slice_apply_plan_ws(B, H, W, gh, gw, gd, 3, 3, 1, int(with_ws), ctypes.byref(v),
+                                                      ctypes.byref(c), ctypes.byref(t), ctypes.byref(sm)), "plan")
+    return v.value, t.value, sm.value
+
+
+@pytest.mark.parametrize("shape", [
+    (1, 576, 3840, 16, 16, 8),      # headline rows (>= 2 Mi px: a workspace is lent)
+    (1, 576, 3840, 32, 32, 16),     # largest grid of the sweep
+    (1, 1024, 2052, 5, 7, 3),       # 1008-byte slab rows
+    (1, 1080, 1920, 16, 16, 8),     # 1080p: no workspace
+    (1, 300, 1917, 16, 16, 8),      # odd width
+    (2, 1080, 1920, 16, 96, 16),    # workspace lent, but no row kernel fits the grid rows
+], ids=lambda s: "x".join(map(str, s)))
+def test_auto_runs_the_kernel_the_plan_reports(shape):
+    """hdrnet_slice_apply_plan_ws describes the call bilateral_slice_apply makes (a workspace lent from
+    2 Mi pixels on): the kernels AUTO launches, read from the profiler, are the ones it reports."""
+    B, H, W, gh, gw, gd = shape
+    variant, threads, smem = plan(*shape, W % 4 == 0 and B * H * W >= (1 << 21))
+    grid, guide, inp = rand_case(61, *shape, signed=True)
+    g, u, i = cuda(grid), cuda(guide), cuda(inp)
+    hdrnet_ops.bilateral_slice_apply(g, u, i, True)    # first launches load modules outside the profile
+    names = launched_kernels(lambda: hdrnet_ops.bilateral_slice_apply(g, u, i, True))
+    want = {_lib.VARIANT_TEX_ASYNC: f"slice_apply_rows_async_kernel<5, (true|false), {threads}, 2, {str(threads == 384).lower()}>",
+            _lib.VARIANT_TEX: rf"slice_apply_rows_tma_kernel<hdrnet_b200::GuideFromInput, 4, 2, {threads}, 0, 0>",
+            _lib.VARIANT_TMA: rf"slice_apply_rows_tma_kernel<hdrnet_b200::GuideFromInput, 0, 2, {threads}, 0, 0>",
+            _lib.VARIANT_GENERIC: "slice_rows_any_kernel<true," if smem else r"slice_generic_kernel<true>"}[variant]
+    pre_pass = variant == _lib.VARIANT_TEX or (variant == _lib.VARIANT_TEX_ASYNC and threads == 352)
+    main = [n for n in names if "yblend_rows_kernel" not in n]
+    assert len(main) == 1 and re.search(want, main[0]), (shape, variant, threads, names)
+    assert len(names) - len(main) == int(pre_pass), names
 
 
 def test_empty_batch_is_a_no_op():

@@ -1,11 +1,10 @@
-"""Same-box A/B of builds / knob settings of libhdrnet_b200.so at the headline shape (box-to-box
+"""Same-box A/B of builds and kernel variants of libhdrnet_b200.so at the headline shape (box-to-box
 spread is +-4 %, larger than most kernel changes).
-    python tools/ab_lib.py SPEC [SPEC ...]      SPEC = path.so[:variant[:KEY=VAL,KEY=VAL...]]
+    python tools/ab_lib.py SPEC [SPEC ...]      SPEC = path.so[:variant]
 Every configuration is driven directly through the C-ABI (hdrnet_slice_apply_f32_ws) in
 interleaved bursts; all burst times and the SM clock sampled after each burst are printed, the
-median is reported.  Outputs of all configurations must be bitwise equal.
-The library reads its tuning record (HDRNET_ASYNC_THREADS, HDRNET_TEX_CHUNKS) ONCE per loaded copy,
-on its first call: every SPEC gets a private copy of the .so, first called under its own settings."""
+median is reported.  Outputs of all configurations must be bitwise equal.  Every library path is
+loaded from a private copy, so two builds at the same path name stay apart."""
 import ctypes, os, shutil, statistics, sys, tempfile, torch
 try:
     import pynvml
@@ -22,15 +21,13 @@ gen = torch.Generator(device="cuda").manual_seed(1234)
 grid = torch.rand(B, GH, GW, GD, 12, device="cuda", generator=gen)
 guide = torch.rand(B, H, W, device="cuda", generator=gen)
 inp = torch.rand(B, H, W, 3, device="cuda", generator=gen)
-KNOBS = ("HDRNET_TEX_CHUNKS", "HDRNET_ASYNC_THREADS", "HDRNET_FUSED_ASYNC", "HDRNET_ASYNC_SLAB")
 libs, cfgs = {}, []
 _tmp = tempfile.mkdtemp(prefix="ab_lib_")
 for spec in sys.argv[1:]:
     parts = spec.split(":")
     path = parts[0]
     variant = int(parts[1]) if len(parts) > 1 and parts[1] else 0
-    env = dict(kv.split("=") for kv in parts[2].split(",")) if len(parts) > 2 and parts[2] else {}
-    if spec not in libs:
+    if path not in libs:
         private = os.path.join(_tmp, f"lib{len(libs)}.so")
         shutil.copy(os.path.abspath(path), private)
         lib = ctypes.CDLL(private)
@@ -38,8 +35,8 @@ for spec in sys.argv[1:]:
         lib.hdrnet_slice_apply_workspace_bytes.argtypes = [ctypes.c_int] * 4
         lib.hdrnet_slice_apply_f32_ws.restype = ctypes.c_int
         lib.hdrnet_slice_apply_f32_ws.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int] * 10 + [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-        libs[spec] = lib
-    cfgs.append((spec, libs[spec], variant, env))
+        libs[path] = lib
+    cfgs.append((spec, libs[path], variant))
 n_ws = next(iter(libs.values())).hdrnet_slice_apply_workspace_bytes(B, H, GW, GD)
 ws = torch.empty(n_ws, dtype=torch.uint8, device="cuda")
 out = torch.empty_like(inp)
@@ -47,14 +44,12 @@ ref = None
 stream = torch.cuda.current_stream().cuda_stream
 
 def run(cfg):
-    _, lib, variant, _ = cfg
+    _, lib, variant = cfg
     rc = lib.hdrnet_slice_apply_f32_ws(grid.data_ptr(), guide.data_ptr(), inp.data_ptr(), out.data_ptr(),
                                        B, H, W, GH, GW, GD, 3, 3, 1, variant, ws.data_ptr(), n_ws, stream)
     assert rc == 0, (cfg[0], rc)
 
 def burst(cfg, iters=40):
-    for k in KNOBS: os.environ.pop(k, None)
-    os.environ.update(cfg[3])
     for _ in range(3): run(cfg)
     torch.cuda.synchronize()
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -65,8 +60,6 @@ def burst(cfg, iters=40):
 
 equal = True
 for cfg in cfgs:   # correctness first: every configuration produces the same bits
-    for k in KNOBS: os.environ.pop(k, None)
-    os.environ.update(cfg[3])
     out.zero_(); run(cfg); torch.cuda.synchronize()
     if ref is None: ref = out.clone()
     elif not torch.equal(ref, out): equal = False; print("MISMATCH:", cfg[0], float((ref - out).abs().max()))

@@ -1,13 +1,11 @@
-"""Times the model path's full-resolution stage (guide + slice + apply in one kernel) at 4K x 8 under
-the CURRENT environment (HDRNET_FUSED_ASYNC = unset / 0 / 1 is read once per process):
-    for f in "" 0 1; do HDRNET_FUSED_ASYNC=$f python tools/time_fused.py; done"""
+"""Times the model path's full-resolution stage (guide + slice + apply in one kernel) at 4K x 8:
+    python tools/time_fused.py
+HDRNET_LIB_OVERRIDE=path.so times another build of the library instead."""
 import os, sys, statistics, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from hdrnet_b200 import models, _lib
 if os.environ.get("HDRNET_LIB_OVERRIDE"):      # another build of the library, for an A/B
     _lib.LIB_PATH = os.path.abspath(os.environ["HDRNET_LIB_OVERRIDE"])
-if os.environ.get("HDRNET_FUSED_ASYNC") == "":
-    del os.environ["HDRNET_FUSED_ASYNC"]
 B, H, W = 8, 2160, 3840
 gen = torch.Generator(device="cuda").manual_seed(1)
 im8 = torch.randint(0, 256, (B, H, W, 3), device="cuda", generator=gen, dtype=torch.uint8)
@@ -32,4 +30,4 @@ for kind, name in (("curves", "HDRNetCurves"), ("nn", "HDRNetPointwiseNNGuide"))
         out[f"{kind} {px}"] = statistics.median(ts)
 import hashlib
 sha = hashlib.sha1(cls._fullres(coeffs, im8, p, torch.uint8).cpu().numpy().tobytes()).hexdigest()[:10]
-print("lib=%s FUSED_ASYNC=%s  u8-sha=%s  " % (os.environ.get("HDRNET_LIB_OVERRIDE", "product"), os.environ.get("HDRNET_FUSED_ASYNC", "unset"), sha) + "  ".join(f"{k}: {v:.4f} ms" for k, v in out.items()))
+print("lib=%s  u8-sha=%s  " % (os.environ.get("HDRNET_LIB_OVERRIDE", "product"), sha) + "  ".join(f"{k}: {v:.4f} ms" for k, v in out.items()))

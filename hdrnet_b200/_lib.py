@@ -45,6 +45,10 @@ SIGNATURES = {
     "hdrnet_slice_apply_plan_ws": (_c_int, [_c_int] * 10 + [ctypes.POINTER(_c_int)] * 4),
     "hdrnet_guide_curves_f32": (_c_int, [_vp, _vp, ctypes.c_longlong] + [_vp] * 5 + [ctypes.c_float, _vp]),
     "hdrnet_guide_nn_f32": (_c_int, [_vp, _vp, ctypes.c_longlong] + [_vp] * 3 + [ctypes.c_float, _c_int, _vp]),
+    # (input, dguide, dinput, npix, ccm, ccm_bias, shifts, slopes, mix, mix_bias, dparams, ws, bytes, stream)
+    "hdrnet_guide_curves_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong]),
+    "hdrnet_guide_curves_grad_f32": (_c_int, [_vp] * 3 + [ctypes.c_longlong] + [_vp] * 5
+                                     + [ctypes.c_float, _vp, _vp, ctypes.c_size_t, _vp]),
     "hdrnet_slice_apply_curves_f32": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 5 + [ctypes.c_float, _vp]),
     "hdrnet_slice_apply_nn_f32": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 3 + [ctypes.c_float, _c_int, _vp]),
     "hdrnet_slice_apply_curves_f32_ws": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 5

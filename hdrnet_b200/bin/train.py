@@ -5,7 +5,7 @@ arguments, flags and defaults (train.py:188-244):
     python -m hdrnet_b200.bin.train <checkpoint_dir> <data_dir> [--eval_data_dir DIR]
         [--learning_rate 1e-4] [--batch_size 16] [--[no]fliplr|flipud|rotate|random_crop]
         [--model_name HDRNetCurves] [--net_input_size 256] [--output_resolution 512 512] ...
-        [--max_steps N] [--seed S]
+        [--max_steps N] [--seed S] [--[no]train_guide]
 
 ``data_dir`` holds ``filelist.txt`` and the ``input/`` and ``output/`` folders (or is that
 ``filelist.txt``); hdrnet_b200/data_pipeline.py keeps the decoded pairs on the device and builds
@@ -24,14 +24,20 @@ directory as it is.  A ``checkpoint_dir`` that already holds a checkpoint is res
 moments and step are restored, and the batches continue where they would have (the sampler is a
 function of ``(seed, step)``).
 
-What is trained: the coefficient network.  The guide's backward, training-mode batch norm and the
-pyramid's resize VJP are not implemented, so ``--batch_norm`` and ``HDRNetGaussianPyrNN`` are
-refused before any data is read, with the models' own ``NotImplementedError``, and the guide
-variables are held fixed at their initial (or restored) values.
+What is trained: the coefficient network, and with ``--train_guide`` the curves guide of
+``HDRNetCurves`` too (``ccm``, ``ccm_bias``, ``shifts``, ``slopes``, ``channel_mixing/*``), in the
+same Adam at the same learning rate, as the reference's single ``opt.minimize`` does
+(train.py:92-94, :115); their Adam slots then go into each checkpoint.  Without the flag (the
+default) the guide variables are held fixed at their initial (or restored) values.  A resume whose
+checkpoint was written with the other setting of the flag is refused before any data is read.
+Training-mode batch norm and the pyramid's resize VJP are not implemented, so ``--batch_norm``,
+``HDRNetGaussianPyrNN`` and ``--train_guide`` with ``HDRNetPointwiseNNGuide`` (whose guide has batch
+norm) are refused before any data is read, with the models' own ``NotImplementedError``.
 
 Deliberate differences from the reference:
 
-* ``--max_steps`` (the reference runs until interrupted) and ``--seed`` are added;
+* ``--max_steps`` (the reference runs until interrupted), ``--seed`` and ``--train_guide`` are added
+  (the reference always trains the guide; here it is opt-in);
   ``--data_pipeline`` takes only ``ImageFilesDataPipeline`` (the tfrecord pipelines need TF);
   ``--profiling`` is accepted and ignored.
 * The evaluation reads ``--eval_data_dir``.  The reference builds the eval pipeline but then
@@ -85,6 +91,9 @@ def build_parser() -> argparse.ArgumentParser:
     train_grp.add_argument("--eval_interval", type=int, default=3600, help="interval between evaluations (in s)")
     train_grp.add_argument("--max_steps", type=int, default=None, help="stop when the global step reaches this (default: run until interrupted).")
     train_grp.add_argument("--seed", type=int, default=0, help="seed of the initial variables and of the data sampler.")
+    train_grp.add_argument("--train_guide", dest="train_guide", action="store_true",
+                           help="train the curves guide's variables too, as the reference does (HDRNetCurves only).")
+    train_grp.add_argument("--notrain_guide", dest="train_guide", action="store_false")
 
     debug_grp = parser.add_argument_group("debug and profiling")
     debug_grp.add_argument("--profiling", dest="profiling", action="store_true", help="accepted for compatibility; ignored.")
@@ -116,7 +125,8 @@ def build_parser() -> argparse.ArgumentParser:
     model_grp.add_argument("--luma_bins", default=8, type=int, help="Number of BGU bins for the luminance.")
     model_grp.add_argument("--spatial_bin", default=16, type=int, help="Size of the spatial BGU bins (pixels).")
 
-    parser.set_defaults(profiling=False, flipud=False, fliplr=False, rotate=False, random_crop=True, batch_norm=False)
+    parser.set_defaults(profiling=False, flipud=False, fliplr=False, rotate=False, random_crop=True, batch_norm=False,
+                        train_guide=False)
     parser.model_group = model_grp
     return parser
 
@@ -126,10 +136,11 @@ def model_params(parser, args) -> dict:
     return {a.dest: getattr(args, a.dest, None) for a in parser.model_group._group_actions}
 
 
-def refuse_untrainable(params) -> None:
-    """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model
-    and training-mode batch norm.  Asks the models themselves, on the CPU, with a stand-in variable
-    that requires grad (they refuse before any device work)."""
+def refuse_untrainable(params, train_guide=False) -> None:
+    """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model,
+    training-mode batch norm and (with ``train_guide``) the pointwise-NN guide.  Asks the models
+    themselves, on the CPU, with a stand-in variable that requires grad (they refuse before any
+    device work)."""
     S = int(params["net_input_size"])
     if params["model_name"] == "HDRNetGaussianPyrNN":
         probe = {COEFFS + "splat/conv1/weights": torch.zeros(1, requires_grad=True)}
@@ -139,6 +150,22 @@ def refuse_untrainable(params) -> None:
         probe = {f"{scope}/BatchNorm/beta": torch.zeros(1, requires_grad=True)
                  for scope, use_bn, _ in models._coefficient_specs(params) if use_bn}
         getattr(models, params["model_name"])._coefficients(torch.zeros(1, S, S, 3), dict(params, weights=probe))
+    if train_guide and params["model_name"] == "HDRNetPointwiseNNGuide":
+        probe = {GUIDE + "conv2/weights": torch.zeros(1, requires_grad=True)}
+        models.HDRNetPointwiseNNGuide.inference(torch.zeros(1, S, S, 3), torch.zeros(1, 1, 1, 3),
+                                                dict(params, weights=probe, guide_grad=True))
+
+
+def refuse_resume_mismatch(saved: dict, train_guide: bool) -> None:
+    """ValueError when a checkpoint to resume was written with the other --[no]train_guide: its guide
+    variables have Adam slots exactly when it trained them."""
+    has_slots = any(k.startswith(GUIDE) and k.endswith(("/Adam", "/Adam_1")) for k in saved)
+    if train_guide and not has_slots:
+        raise ValueError("the checkpoint to resume was trained with the guide held fixed (no Adam slots for "
+                         "inference/guide/*): resume it without --train_guide, or start a new checkpoint_dir")
+    if has_slots and not train_guide:
+        raise ValueError("the checkpoint to resume was trained with --train_guide (it holds Adam slots for "
+                         "inference/guide/*): resume it with --train_guide")
 
 
 def slot_names(name):
@@ -187,7 +214,8 @@ class Trainer:
         self.device = torch.device("cuda", torch.cuda.current_device())
         init = models.init_weights(params, seed=args.seed, model_name=params["model_name"])
         self.weights = {k: torch.from_numpy(v).to(self.device) for k, v in init.items()}
-        self.names = sorted(k for k in self.weights if k.startswith(COEFFS))
+        trained = (COEFFS, GUIDE) if args.train_guide else (COEFFS,)
+        self.names = sorted(k for k in self.weights if k.startswith(trained))
         for k in self.names:
             self.weights[k].requires_grad_(True)
         self.opt = torch.optim.Adam([self.weights[k] for k in self.names], lr=args.learning_rate,
@@ -195,9 +223,13 @@ class Trainer:
         self.step = 0
         self.ema = {"loss": 0.0, "psnr": 0.0}
         self._resume()
-        log.info("%s: training the %d coefficient-network variables; the guide variables (%s*) are held fixed "
-                 "at their %s values", params["model_name"], len(self.names), GUIDE,
-                 "restored" if self.step else "initial")
+        if args.train_guide:
+            log.info("%s: training the %d coefficient-network and guide variables (the guide is trained)",
+                     params["model_name"], len(self.names))
+        else:
+            log.info("%s: training the %d coefficient-network variables; the guide variables (%s*) are held fixed "
+                     "at their %s values", params["model_name"], len(self.names), GUIDE,
+                     "restored" if self.step else "initial")
         self.train_data = data_pipeline.ImageFilesDataPipeline(
             args.data_dir, batch_size=args.batch_size, output_resolution=args.output_resolution, shuffle=True,
             fliplr=args.fliplr, flipud=args.flipud, rotate=args.rotate, random_crop=args.random_crop,
@@ -208,13 +240,17 @@ class Trainer:
                 args.eval_data_dir, batch_size=1, output_resolution=args.output_resolution, shuffle=False,
                 params=params, nthreads=1, device=self.device)
         self.p = dict(params, weights=self.weights)
+        if args.train_guide:
+            self.p["guide_grad"] = True
 
     # ---- checkpoints ---------------------------------------------------------------------------
     def _resume(self):
         prefix = checkpoint.latest_checkpoint(self.args.checkpoint_dir)
         if prefix is None:
             return
-        values, moments, step, ema = restored_state(checkpoint.read_tf_checkpoint(prefix), self.weights, self.names)
+        saved = checkpoint.read_tf_checkpoint(prefix)
+        refuse_resume_mismatch(saved, self.args.train_guide)
+        values, moments, step, ema = restored_state(saved, self.weights, self.names)
         with torch.no_grad():
             for k, v in self.weights.items():
                 v.copy_(torch.from_numpy(values[k]).reshape(v.shape))
@@ -309,7 +345,10 @@ def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
     params = model_params(parser, args)
-    refuse_untrainable(params)                       # before any data is read
+    refuse_untrainable(params, args.train_guide)     # before any data is read
+    prefix = checkpoint.latest_checkpoint(args.checkpoint_dir)
+    if prefix is not None:
+        refuse_resume_mismatch(checkpoint.read_tf_checkpoint(prefix), args.train_guide)
     if args.profiling:
         log.warning("--profiling is accepted for compatibility and ignored")
     if not torch.cuda.is_available():

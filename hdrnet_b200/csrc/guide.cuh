@@ -41,24 +41,33 @@ struct NNGuideParams {
   float b2;
 };
 
-__device__ __forceinline__ float curves_guide(const CurvesGuideParams& p, float r, float g,
-                                              float b) {
+// The curves guide before its clip: returns a = sum_c mix_c * u_c + mix_bias and stores the
+// colour-corrected t_c.  The guide VJP (guide_grad.cu) decides its masks [0 <= a <= 1] and
+// [t_c > shift] from these very floats, so they agree with the forward pixel by pixel.
+__device__ __forceinline__ float curves_guide_preclip(const CurvesGuideParams& p, float r, float g,
+                                                      float b, float t[3]) {
   // One FMNMX and one FFMA per knot (vs FADD + FMNMX + FFMA each).
   float acc = p.folded_bias;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float t = fmaf(b, p.ccm[2][c], fmaf(g, p.ccm[1][c], fmaf(r, p.ccm[0][c], p.ccm_bias[c])));
+    t[c] = fmaf(b, p.ccm[2][c], fmaf(g, p.ccm[1][c], fmaf(r, p.ccm[0][c], p.ccm_bias[c])));
     unsigned long long u2 = 0ull;  // (0.0f, 0.0f)
 #pragma unroll
     for (int k = 0; k < kCurvePts; k += 2) {
-      const unsigned long long m2 = pack2(fmaxf(t, p.shifts[c][k]), fmaxf(t, p.shifts[c][k + 1]));
+      const unsigned long long m2 = pack2(fmaxf(t[c], p.shifts[c][k]), fmaxf(t[c], p.shifts[c][k + 1]));
       u2 = fma2(pack2(p.slopes[c][k], p.slopes[c][k + 1]), m2, u2);
     }
     float u0, u1;
     unpack2(u2, u0, u1);
     acc = fmaf(p.mix[c], u0 + u1, acc);
   }
-  return fminf(fmaxf(acc, 0.0f), 1.0f);
+  return acc;
+}
+
+__device__ __forceinline__ float curves_guide(const CurvesGuideParams& p, float r, float g,
+                                              float b) {
+  float t[3];
+  return fminf(fmaxf(curves_guide_preclip(p, r, g, b, t), 0.0f), 1.0f);
 }
 
 // kFeats is a compile-time bound (16 or 32): the loop unrolls fully and every weight is a

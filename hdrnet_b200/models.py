@@ -22,9 +22,13 @@ autograd Functions over the same forward kernels and the VJP kernels of ``csrc/c
 ``torch.optim`` can fine-tune the network through the slice-apply VJP with the guide held fixed.
 A dict holding tensors is never cached: every call reads the current values.  The gradients are
 those of the inference-form graph; with ``batch_norm=False`` (the reference's default,
-hdrnet/bin/train.py:224-236) that is the coefficient network's training graph.  Guide variables,
-``fullres_input``, batch-norm layers and the pyramid model's resize are not differentiated: asking
-for their gradient raises ``NotImplementedError``.
+hdrnet/bin/train.py:224-236) that is the coefficient network's training graph.  With
+``params['guide_grad']`` truthy, ``HDRNetCurves``'s guide variables (``ccm``, ``ccm_bias``,
+``shifts``, ``slopes``, ``channel_mixing/*``) and ``fullres_input`` are differentiated too, through
+``_CurvesGuideFn`` and the VJP of ``csrc/guide_grad.cu``; without the key, asking for their gradient
+raises ``NotImplementedError`` as before.  The pointwise-NN guide (its conv1 has batch norm, which
+training runs in training mode), batch-norm layers and the pyramid model's resize are not
+differentiated: asking for their gradient raises ``NotImplementedError``.
 
 Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
   coefficients  4 splat convs, 2 global convs + 3 FCs, 2 local convs (conv2d / fc kernels),
@@ -566,6 +570,72 @@ class _FusePredictFn(torch.autograd.Function):
         return dl, dg, dw, db, None, None, None
 
 
+_CURVES_VARS = ("ccm", "ccm_bias", "shifts", "slopes", "channel_mixing/weights", "channel_mixing/biases")
+# [start, end) of each variable in the library's 112-float parameter gradient (include/hdrnet_b200.h)
+_CURVES_GRAD_SLICES = ((0, 9), (9, 12), (12, 60), (60, 108), (108, 111), (111, 112))
+
+
+def _host_f32(v) -> np.ndarray:
+    a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+    return np.ascontiguousarray(a, np.float32).reshape(-1)
+
+
+class _CurvesGuideFn(torch.autograd.Function):
+    """The curves guide (hdrnet/models.py:145-190) over its six variables (_CURVES_VARS order):
+    forward hdrnet_guide_curves_f32, the standalone guide kernel (the guide keeps its bits),
+    backward hdrnet_guide_curves_grad_f32 with the host copies of the variables the forward used."""
+
+    @staticmethod
+    def forward(ctx, x, ccm, ccm_bias, shifts, slopes, mix, mix_bias):
+        x = x.contiguous()
+        host = [_host_f32(v) for v in (ccm, ccm_bias, shifts, slopes, mix, mix_bias)]
+        B, H, W, _ = x.shape
+        guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device):
+            rc = _lib.load().hdrnet_guide_curves_f32(
+                x.data_ptr(), guide.data_ptr(), B * H * W, *[_hp(a) for a in host[:5]], float(host[5][0]),
+                _stream(x.device))
+        _lib.check(rc, "guide_curves")
+        ctx.save_for_backward(x)
+        ctx.host = host
+        ctx.vars = [(v.shape, v.device) if isinstance(v, torch.Tensor) else None
+                    for v in (ccm, ccm_bias, shifts, slopes, mix, mix_bias)]
+        return guide
+
+    @staticmethod
+    def backward(ctx, dguide):
+        (x,) = ctx.saved_tensors
+        dguide = dguide.contiguous()
+        need_x = ctx.needs_input_grad[0]
+        need_p = any(ctx.needs_input_grad[1:])
+        B, H, W, _ = x.shape
+        npix = B * H * W
+        dx = torch.empty_like(x) if need_x else None
+        dp = torch.empty(112, dtype=torch.float32, device=x.device) if need_p else None
+        lib = _lib.load()
+        ws = _grad_workspace(x.device, lib.hdrnet_guide_curves_grad_workspace_bytes(npix)) if need_p else None
+        host = ctx.host
+        with torch.cuda.device(x.device):
+            rc = lib.hdrnet_guide_curves_grad_f32(
+                x.data_ptr(), dguide.data_ptr(), _ptr(dx), npix, *[_hp(a) for a in host[:5]], float(host[5][0]),
+                _ptr(dp), _ptr(ws), 0 if ws is None else ws.numel() * 4, _stream(x.device))
+        _lib.check(rc, "guide_curves VJP")
+        grads = []
+        for need, var, (a, b) in zip(ctx.needs_input_grad[1:], ctx.vars, _CURVES_GRAD_SLICES):
+            # a copy per variable: optimizers may update a .grad in place
+            grads.append(dp[a:b].reshape(var[0]).to(var[1], copy=True) if need and var is not None else None)
+        return (dx, *grads)
+
+
+def _curves_guide_grad(wts, params, x) -> bool:
+    """Whether HDRNetCurves._guide goes through autograd: grad enabled, params['guide_grad'] truthy,
+    and a guide variable or the input requiring grad."""
+    if not (torch.is_grad_enabled() and isinstance(params, dict) and params.get("guide_grad")):
+        return False
+    return _requires_grad(x) or (wts is not None and
+                                 any(_requires_grad(wts.get("inference/guide/" + n)) for n in _CURVES_VARS))
+
+
 def _requires_grad(t) -> bool:
     return isinstance(t, torch.Tensor) and t.requires_grad
 
@@ -574,9 +644,10 @@ def _trainable_keys(wts, prefix: str):
     return sorted(k for k, v in wts.items() if k.startswith(prefix) and _requires_grad(v))
 
 
-def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None) -> None:
+def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None, nn_guide=False) -> None:
     """NotImplementedError for every gradient this package does not compute (checked before any
-    device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN)."""
+    device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN).  The curves
+    guide's variables and fullres_input are differentiated only with params['guide_grad']."""
     if not torch.is_grad_enabled() or wts is None:
         return
     if what is not None:
@@ -587,12 +658,21 @@ def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=N
                                       "its _coefficients is differentiable on its own")
         return
     guide = _trainable_keys(wts, "inference/guide")
-    if guide:
+    guide_grad = bool(params.get("guide_grad")) if isinstance(params, dict) else False
+    if guide_grad and nn_guide and (guide or _requires_grad(fullres_input)):
+        wanted = guide[0] if guide else "fullres_input"
+        raise NotImplementedError(
+            f"gradients for the pointwise-NN guide variables and its fullres_input are not implemented ({wanted} "
+            "requires grad): its conv1 has batch norm, which training runs in training mode with batch "
+            "statistics, a different forward")
+    hint = "; params['guide_grad'] computes them for HDRNetCurves"
+    if guide and not guide_grad:
         raise NotImplementedError(f"gradients for the guide variables are not implemented ({guide[0]} requires "
-                                  "grad): the guide is held fixed; set requires_grad=False on its variables")
-    if _requires_grad(fullres_input):
+                                  "grad): the guide is held fixed; set requires_grad=False on its variables"
+                                  + ("" if nn_guide else hint))
+    if _requires_grad(fullres_input) and not guide_grad:
         raise NotImplementedError("gradients for fullres_input are not implemented: they need the guide's "
-                                  "backward; pass it with requires_grad=False")
+                                  "backward; pass it with requires_grad=False" + ("" if nn_guide else hint))
     _refuse_batch_norm(wts, params)
 
 
@@ -633,14 +713,18 @@ class HDRNetCurves(object):
         ``cls.last_debug`` (the collections run.py --debug reads, run.py:98-133).
 
         With coefficient-network variables (or lowres_input) requiring grad, the coefficients come
-        from autograd and the output from the standalone guide kernel (a constant) and
-        hdrnet_ops.bilateral_slice_apply, whose VJP carries the gradient back to the grid."""
+        from autograd and the output from the standalone guide kernel and
+        hdrnet_ops.bilateral_slice_apply, whose VJP carries the gradient back to the grid.  The guide
+        is a constant there unless params['guide_grad'] is truthy and a curves-guide variable or
+        fullres_input requires grad: then it is _CurvesGuideFn, whose VJP takes the slice-apply's
+        guide gradient to the guide variables and adds its input gradient to the slice-apply's."""
         if is_training:
             raise NotImplementedError("hdrnet_b200 implements the inference path only")
-        _refuse_untrained(_weights_or_none(params), params, fullres_input=fullres_input)
+        wts = _weights_or_none(params)
+        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=bool(cls._nn_guide))
         fullres_input = _check_input(fullres_input, "fullres_input")
         coeffs = cls._coefficients(lowres_input, params, is_training)
-        if coeffs.requires_grad:
+        if coeffs.requires_grad or (not cls._nn_guide and _curves_guide_grad(wts, params, fullres_input)):
             with torch.cuda.device(fullres_input.device):
                 guide = cls._guide(fullres_input, params)
             B, gh, gw, gd = coeffs.shape[:4]
@@ -819,9 +903,14 @@ class HDRNetCurves(object):
 
     @classmethod
     def _guide(cls, input_tensor, params, is_training=False):
-        """models.py:145-190 as a standalone kernel -> [B, H, W]."""
+        """models.py:145-190 as a standalone kernel -> [B, H, W].  Differentiable (_CurvesGuideFn)
+        when _curves_guide_grad says so."""
         x = _check_input(input_tensor, "fullres_input")
-        prep = _prepare(_resolve_weights(params), params, x.device, False)
+        wts = _resolve_weights(params)
+        if _curves_guide_grad(wts, params, x):
+            with torch.cuda.device(x.device):
+                return _CurvesGuideFn.apply(x, *[wts["inference/guide/" + n] for n in _CURVES_VARS])
+        prep = _prepare(wts, params, x.device, False)
         B, H, W, _ = x.shape
         guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):

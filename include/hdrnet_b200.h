@@ -209,6 +209,31 @@ HDRNET_API int hdrnet_guide_nn_f32(const float* input, float* guide, long long n
                                    int feats, void* stream);
 
 /*
+ * Curves-guide VJP: the backward of hdrnet_guide_curves_f32 (training the guide; the gradient TF
+ * gives HDRNetCurves._guide, hdrnet/models.py:145-190).  dguide [npix] is the gradient of the
+ * guide; the clip passes it where 0 <= a <= 1 (equality included, as tf.clip_by_value) and each
+ * relu where t > shift (0 at equality, as TF's ReluGrad), both decided on the forward's own floats.
+ *   dinput [npix, 3]  gradient of the input; NULL: not computed.
+ *   dparams [112]     DEVICE array, the gradients of the variables summed over all npix pixels, in
+ *                     the order ccm 9 ([in][out]), ccm_bias 3, shifts 48 ([3][16]), slopes 48
+ *                     ([3][16]), mix 3, mix_bias 1; NULL: not computed.
+ * The coefficient arrays are HOST pointers, as for hdrnet_guide_curves_f32.  Gradients are written,
+ * not accumulated.  The parameter sums go through per-CTA partial sums of fixed pixel chunks (the
+ * chunk size depends on npix alone) in a caller-lent workspace of
+ * hdrnet_guide_curves_grad_workspace_bytes(npix) bytes (needed when dparams is not NULL; smaller:
+ * HDRNET_E_BAD_SHAPE), then a second pass adds the chunks in a fixed order: no atomics, bitwise
+ * reproducible.  The workspace is scratch, undefined after the call.  npix == 0 writes zero
+ * parameter gradients.
+ */
+HDRNET_API size_t hdrnet_guide_curves_grad_workspace_bytes(long long npix);
+HDRNET_API int hdrnet_guide_curves_grad_f32(const float* input, const float* dguide, float* dinput,
+                                            long long npix, const float* ccm,
+                                            const float* ccm_bias, const float* shifts,
+                                            const float* slopes, const float* mix, float mix_bias,
+                                            float* dparams, void* workspace,
+                                            size_t workspace_bytes, void* stream);
+
+/*
  * Model-path forms of slice-apply: the guide is computed per pixel INSIDE the kernel from the
  * full-res RGB (the guide map never touches HBM: 24 B/px instead of 28 B/px + a guide pass).
  * Replaces HDRNetCurves.inference / HDRNetPointwiseNNGuide.inference's `_guide` + `_output`

@@ -1,0 +1,403 @@
+"""GPU tests of the curves-guide VJP (csrc/guide_grad.cu, models._CurvesGuideFn) against the
+float64 reference (oracle/guide_f64.py): shapes from 7 x 5 to a 4K frame, unaligned buffers, the
+tie known answers, dinput / dparams NULL, bitwise repeatability, the buffer contract; then the model
+with params['guide_grad'] at the training size against the float64 chain, the unchanged forward, and
+a teacher whose guide differs from the student's."""
+import ctypes
+
+import numpy as np
+import pytest
+import torch
+
+from hdrnet_b200 import _lib, models
+from oracle import cnn_grad_f64 as C
+from oracle import guide_f64, slice_f64
+
+pytestmark = pytest.mark.gpu
+
+G = "inference/guide"
+DX_BAR = 1e-5       # dinput: max |diff| / max |ref|
+P_BAR = 4e-6        # every parameter-gradient element: |diff| / Σ|terms|
+
+
+def report(what, **vals):
+    print("MEASURE", what, " ".join(f"{k}={v:.3g}" if isinstance(v, float) else f"{k}={v}"
+                                    for k, v in vals.items()), flush=True)
+
+
+def np_(t):
+    return t.detach().cpu().numpy()
+
+
+def cuda(a, grad=False):
+    return torch.from_numpy(np.ascontiguousarray(np.asarray(a, np.float32))).cuda().requires_grad_(grad)
+
+
+def guide_weights(rng, spread=0.3):
+    """Curves-guide variables (float32, model shapes) well away from the identity-like initial curve."""
+    w = {f"{G}/ccm": np.eye(3) + spread * rng.randn(3, 3),
+         f"{G}/ccm_bias": 0.1 * rng.randn(3),
+         f"{G}/shifts": np.sort(rng.rand(1, 1, 3, 16), axis=-1),
+         f"{G}/slopes": rng.randn(1, 1, 1, 3, 16) * 0.5,
+         f"{G}/channel_mixing/weights": rng.rand(1, 1, 3, 1) * 0.6,
+         f"{G}/channel_mixing/biases": np.array([0.1])}
+    return {k: np.asarray(v, np.float32) for k, v in w.items()}
+
+
+def host(w):
+    a = [np.ascontiguousarray(np.asarray(w[f"{G}/{n}"], np.float32).reshape(-1)) for n in guide_f64.NAMES]
+    return a[:5], float(a[5][0])
+
+
+def hp(a):
+    return a.ctypes.data_as(ctypes.c_void_p)
+
+
+def vjp_cuda(x, g, w, want_dx=True, want_p=True, ws=None, dx=None, dp=None):
+    """The C-ABI on device tensors x [..., 3] and g [...] (views allowed); returns (dx, dp)."""
+    lib = _lib.load()
+    npix = g.numel()
+    arrs, mix_bias = host(w)
+    if want_dx and dx is None:
+        dx = torch.empty_like(x)
+    if want_p and dp is None:
+        dp = torch.empty(112, dtype=torch.float32, device="cuda")
+    nbytes = lib.hdrnet_guide_curves_grad_workspace_bytes(npix)
+    if want_p and ws is None:
+        ws = torch.empty(max(nbytes, 4) // 4, dtype=torch.float32, device="cuda")
+    rc = lib.hdrnet_guide_curves_grad_f32(
+        x.data_ptr(), g.data_ptr(), dx.data_ptr() if want_dx else None, npix, *[hp(a) for a in arrs], mix_bias,
+        dp.data_ptr() if want_p else None, ws.data_ptr() if want_p else None, nbytes if want_p else 0,
+        torch.cuda.current_stream().cuda_stream)
+    _lib.check(rc, "guide_curves VJP")
+    torch.cuda.synchronize()
+    return (dx if want_dx else None), (dp if want_p else None)
+
+
+def safe_dguide(x, g, w):
+    """g with 0 where the float32 forward's mask could differ from the float64 one: t within a few
+    ulp of a knot, or a within a few ulp of 0 or 1.  Returns (g, number of such pixels)."""
+    a, t = guide_f64.preclip(x, w)
+    s = np.asarray(w[f"{G}/shifts"], np.float64).reshape(3, 16)
+    near_t = (np.abs(t[..., None] - s) <= 1e-6 * np.maximum(1.0, np.abs(t[..., None]))).any(axis=(-1, -2))
+    near_a = (np.abs(a) <= 1e-5) | (np.abs(a - 1.0) <= 1e-5)
+    near = near_t | near_a
+    return np.where(near, 0.0, g).astype(np.float32), int(near.sum())
+
+
+def check(what, x, g, w, dx, dp):
+    ref = guide_f64.vjp(x, g, w)
+    errs = {}
+    if dx is not None:
+        e = np.abs(np_(dx).astype(np.float64) - ref.dinput).max() / max(np.abs(ref.dinput).max(), 1e-30)
+        errs["dinput"] = float(e)
+        assert e <= DX_BAR, f"{what} dinput: {e:.3e} of range"
+    if dp is not None:
+        got, want, terms = np_(dp).astype(np.float64), guide_f64.flat(ref.dparams), guide_f64.flat(ref.dparams_abs)
+        e = np.abs(got - want) / np.maximum(terms, 1e-30)
+        e[(terms == 0) & (got == 0)] = 0.0
+        errs["params"] = float(e.max())
+        assert e.max() <= P_BAR, f"{what} dparams[{int(e.argmax())}]: {e.max():.3e} of Σ|terms|"
+    return errs
+
+
+SHAPES = [(1, 5, 7), (1, 1, 1), (2, 3, 5), (3, 17, 31), (16, 512, 512), (1, 2160, 3840)]
+
+
+@pytest.mark.parametrize("shape", SHAPES, ids=lambda s: "x".join(map(str, s)))
+def test_vjp_matches_float64(shape):
+    rng = np.random.RandomState(sum(shape))
+    w = guide_weights(rng)
+    x = (rng.rand(*shape, 3) * 1.2 - 0.1).astype(np.float32)
+    g, near = safe_dguide(x, rng.randn(*shape), w)
+    npix = int(np.prod(shape))
+    report(f"guide VJP {shape}", near_tie_pixels=near, of=npix)
+    assert near <= max(2, npix // 2000)
+    dx, dp = vjp_cuda(cuda(x), cuda(g), w)
+    report(f"guide VJP {shape}", **check(str(shape), x, g, w, dx, dp))
+
+
+@pytest.mark.parametrize("offset", [1, 2, 3], ids=lambda o: f"{4 * o}B")
+def test_unaligned_buffers(offset):
+    rng = np.random.RandomState(offset)
+    w = guide_weights(rng)
+    n = 3001
+    x = rng.rand(n, 3).astype(np.float32)
+    g, _ = safe_dguide(x, rng.randn(n), w)
+    xb = torch.zeros(3 * n + 3 * offset + 4, device="cuda")
+    gb = torch.zeros(n + offset + 4, device="cuda")
+    db = torch.zeros(3 * n + 3 * offset + 4, device="cuda")
+    xv = xb[offset:offset + 3 * n]
+    xv.copy_(cuda(x).reshape(-1))
+    gv = gb[offset:offset + n]
+    gv.copy_(cuda(g))
+    dv = db[offset:offset + 3 * n]
+    dx, dp = vjp_cuda(xv, gv, w, dx=dv)
+    check(f"offset {4 * offset} B", x, g, w, dx.reshape(n, 3), dp)
+    aligned = vjp_cuda(cuda(x), cuda(g), w)
+    assert torch.equal(dx.reshape(n, 3), aligned[0])     # dinput is per pixel: the same bits either way
+
+
+def tie_weights(slopes, mix_bias=0.0):
+    return {f"{G}/ccm": np.eye(3, dtype=np.float32), f"{G}/ccm_bias": np.zeros(3, np.float32),
+            f"{G}/shifts": np.tile(np.arange(16, dtype=np.float32) / 16, (1, 1, 3, 1)),
+            f"{G}/slopes": np.asarray(slopes, np.float32).reshape(1, 1, 1, 3, 16),
+            f"{G}/channel_mixing/weights": np.array([1, 0, 0], np.float32).reshape(1, 1, 3, 1),
+            f"{G}/channel_mixing/biases": np.array([mix_bias], np.float32)}
+
+
+def test_tie_known_answers_on_the_device():
+    """The known answers of tests/test_guide_f64.py, now from the kernel: x_0 = 0.25 = s_4 exactly
+    (all slopes 1), and a = 0, a = 1 exactly, a < 0 and a > 1 (slope 1 on knot 0)."""
+    w = tie_weights(np.ones(48))
+    x = np.array([[0.25, 0.5, 0.7]], np.float32)
+    dx, dp = vjp_cuda(cuda(x), cuda([2.0]), w)
+    ref = guide_f64.vjp(x, [2.0], w)
+    assert np.array_equal(np_(dx), ref.dinput.astype(np.float32))
+    assert np.allclose(np_(dp), guide_f64.flat(ref.dparams), rtol=1e-6, atol=0)
+    assert np.array_equal(np_(dp)[12:28], [-2.0] * 4 + [0.0] * 12)        # no gradient for the knot at t
+    slopes = np.zeros(48)
+    slopes[0] = 1
+    for x0, mb in ((0.0, 0.0), (1.0, 0.0), (0.25, -0.5), (1.5, 0.0)):
+        w = tie_weights(slopes, mb)
+        x = np.array([[x0, 0.3, 0.6]], np.float32)
+        dx, dp = vjp_cuda(cuda(x), cuda([3.0]), w)
+        ref = guide_f64.vjp(x, [3.0], w)
+        assert np.array_equal(np_(dx), ref.dinput.astype(np.float32)), (x0, mb)
+        assert np.allclose(np_(dp), guide_f64.flat(ref.dparams), rtol=1e-6, atol=0), (x0, mb)
+        assert (np_(dp)[111] == 3.0) == (mb == 0.0 and x0 <= 1.0)            # the clip passes at 0 and 1
+
+
+def test_null_outputs_and_repeatability():
+    rng = np.random.RandomState(9)
+    w = guide_weights(rng)
+    x = rng.rand(4, 130, 257, 3).astype(np.float32)
+    g, _ = safe_dguide(x, rng.randn(4, 130, 257), w)
+    tx, tg = cuda(x), cuda(g)
+    dx, dp = vjp_cuda(tx, tg, w)
+    dx_only, _ = vjp_cuda(tx, tg, w, want_p=False)
+    _, dp_only = vjp_cuda(tx, tg, w, want_dx=False)
+    assert torch.equal(dx_only, dx) and torch.equal(dp_only, dp)
+    for _ in range(2):
+        again = vjp_cuda(tx, tg, w)
+        assert torch.equal(again[0], dx) and torch.equal(again[1], dp)
+    lib = _lib.load()
+    arrs, mb = host(w)
+    assert lib.hdrnet_guide_curves_grad_f32(tx.data_ptr(), tg.data_ptr(), None, tg.numel(), *[hp(a) for a in arrs],
+                                            mb, None, None, 0, None) == _lib.OK
+    zero = torch.full((112,), 7.0, device="cuda")
+    assert lib.hdrnet_guide_curves_grad_f32(None, None, None, 0, *[hp(a) for a in arrs], mb, zero.data_ptr(),
+                                            None, 0, None) == _lib.OK
+    torch.cuda.synchronize()
+    assert not zero.any()                                                     # npix == 0: zero gradients
+
+
+def test_buffer_contract():
+    """Guarded views, the workspace lent at exactly its queried size and pre-filled with 0xFF and
+    then 0x5A: the outputs are the same either way, nothing outside the views is written, and one
+    byte less of workspace is refused."""
+    rng = np.random.RandomState(11)
+    w = guide_weights(rng)
+    n = 2 * 67 * 129 + 3
+    x = rng.rand(n, 3).astype(np.float32)
+    g, _ = safe_dguide(x, rng.randn(n), w)
+    lib = _lib.load()
+    nbytes = lib.hdrnet_guide_curves_grad_workspace_bytes(n)
+    guard = 64
+    outs = []
+    for fill in (0xFF, 0x5A):
+        ws = torch.full((nbytes + 2 * guard,), fill, dtype=torch.uint8, device="cuda")
+        dxb = torch.full((3 * n + 2 * guard,), float("nan"), device="cuda")
+        dpb = torch.full((112 + 2 * guard,), float("nan"), device="cuda")
+        xb = torch.full((3 * n + 2 * guard,), float("nan"), device="cuda")
+        xb[guard:guard + 3 * n] = cuda(x).reshape(-1)
+        gb = torch.full((n + 2 * guard,), float("nan"), device="cuda")
+        gb[guard:guard + n] = cuda(g)
+        arrs, mb = host(w)
+        rc = lib.hdrnet_guide_curves_grad_f32(
+            xb[guard:].data_ptr(), gb[guard:].data_ptr(), dxb[guard:].data_ptr(), n, *[hp(a) for a in arrs], mb,
+            dpb[guard:].data_ptr(), ws[guard:].data_ptr(), nbytes, None)
+        assert rc == _lib.OK
+        torch.cuda.synchronize()
+        for buf, size in ((dxb, 3 * n), (dpb, 112)):
+            assert torch.isnan(buf[:guard]).all() and torch.isnan(buf[guard + size:]).all()
+            assert not torch.isnan(buf[guard:guard + size]).any()
+        assert (ws[:guard] == fill).all() and (ws[guard + nbytes:] == fill).all()
+        outs.append((dxb[guard:guard + 3 * n].clone(), dpb[guard:guard + 112].clone()))
+        assert lib.hdrnet_guide_curves_grad_f32(
+            xb[guard:].data_ptr(), gb[guard:].data_ptr(), None, n, *[hp(a) for a in arrs], mb,
+            dpb[guard:].data_ptr(), ws[guard:].data_ptr(), nbytes - 1, None) == _lib.E_BAD_SHAPE
+    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
+    check("buffer contract", x, g, w, outs[0][0].reshape(n, 3), outs[0][1])
+
+
+# ---- the model -----------------------------------------------------------------------------------
+TRAIN = dict(models.DEFAULT_PARAMS)
+
+
+def model_weights(seed, grad_coeffs=True, grad_guide=True):
+    rng = np.random.RandomState(seed)
+    w = models.init_weights(TRAIN, seed=seed)
+    w.update(guide_weights(rng, spread=0.15))
+    w[f"{G}/shifts"] = np.sort(rng.rand(1, 1, 3, 16), axis=-1).astype(np.float32) * 0.9
+    w[f"{G}/slopes"] = (np.abs(rng.randn(1, 1, 1, 3, 16)) * 0.3).astype(np.float32)
+    out = {}
+    for k, v in w.items():
+        if k.endswith("/biases") and k.startswith(C.P):
+            v = (0.05 * rng.randn(*v.shape)).astype(np.float32)
+        grad = grad_coeffs if k.startswith(C.P) else grad_guide
+        out[k] = torch.from_numpy(v).cuda().requires_grad_(grad)
+    return out
+
+
+def coefficient_grads_f64(low, wts, dgrid):
+    """float64 VJPs of every coefficient layer (cnn_grad_f64's per-layer VJPs) chained back from
+    dgrid, each fed the CUDA forward's own activations, so that no ReLU mask flipped by rounding
+    decides a comparison."""
+    P = C.P
+    L = {s: (wts[s + "/weights"].detach(), None if wts.get(s + "/biases") is None else wts[s + "/biases"].detach())
+         for s, _, _ in models._coefficient_specs(TRAIN)}
+    acts = {}
+
+    def conv(s, x, stride, relu):
+        acts[s] = (x, models._ConvFn.apply(x, *L[s], stride, relu), stride, relu)
+        return acts[s][1]
+
+    def fc(s, x, relu):
+        acts[s] = (x, models._FcFn.apply(x, *L[s], relu), None, relu)
+        return acts[s][1]
+
+    with torch.no_grad():
+        x = low
+        for i in range(4):
+            x = conv(f"{P}/splat/conv{i + 1}", x, 2, True)
+        splat = x
+        g2 = conv(f"{P}/global/conv2", conv(f"{P}/global/conv1", splat, 2, True), 2, True)
+        g = fc(f"{P}/global/fc3", fc(f"{P}/global/fc2", fc(f"{P}/global/fc1", g2.reshape(16, -1), True), True), False)
+        loc = conv(f"{P}/local/conv2", conv(f"{P}/local/conv1", splat, 1, True), 1, False)
+    grads = {}
+    wp = np_(L[f"{P}/prediction/conv1"][0])
+    v = C.fuse_predict_vjp(np_(loc), np_(g), wp[0, 0], dgrid, 8, 3, 4)
+    grads[f"{P}/prediction/conv1/weights"], grads[f"{P}/prediction/conv1/biases"] = v.dw.reshape(wp.shape), v.db
+
+    def back(s, dy):
+        x, out, stride, relu = acts[s]
+        w = np_(L[s][0])
+        r = C.fc_vjp(np_(x), w, np_(out), dy, relu) if stride is None else C.conv_vjp(np_(x), w, np_(out), dy, stride, relu)
+        grads[s + "/weights"] = r.dw
+        if L[s][1] is not None:
+            grads[s + "/biases"] = r.db
+        return r.dx
+
+    dsplat = back(f"{P}/local/conv1", back(f"{P}/local/conv2", v.dlocal))
+    d = back(f"{P}/global/fc1", back(f"{P}/global/fc2", back(f"{P}/global/fc3", v.dglobal)))
+    dsplat = dsplat + back(f"{P}/global/conv1", back(f"{P}/global/conv2", d.reshape(g2.shape)))
+    for i in reversed(range(4)):
+        dsplat = back(f"{P}/splat/conv{i + 1}", dsplat)
+    return grads
+
+
+def test_model_gradients_at_training_size_match_the_float64_chain():
+    """L2 loss of HDRNetCurves.inference at 16 x 512² with guide_grad, back to every coefficient
+    variable, every guide variable and fullres_input; float64: slice_f64 (with the CUDA guide) gives
+    the grid, guide and input VJPs, cnn_grad_f64's layer VJPs the network's, guide_f64 the guide's."""
+    wts = model_weights(2)
+    rng = np.random.RandomState(3)
+    low = rng.rand(16, 256, 256, 3).astype(np.float32)
+    full = rng.rand(16, 512, 512, 3).astype(np.float32)
+    params = dict(TRAIN, weights=wts, guide_grad=True)
+    tf = cuda(full, True)
+    out = models.HDRNetCurves.inference(cuda(low), tf, params)
+    wn = {k: np_(v) for k, v in wts.items()}
+    # a zero output gradient where a mask is decided by rounding (as safe_dguide)
+    keep = np.ones(full.shape[:3], np.float32)
+    a, t = guide_f64.preclip(full, wn)
+    s = wn[f"{G}/shifts"].astype(np.float64).reshape(3, 16)
+    mask = (np.abs(t[..., None] - s) <= 1e-6 * np.maximum(1.0, np.abs(t[..., None]))).any(axis=(-1, -2)) | \
+        (np.abs(a) <= 1e-5) | (np.abs(a - 1.0) <= 1e-5)
+    keep[mask] = 0.0
+    report("model near-tie pixels", count=int(mask.sum()), of=int(mask.size))
+    assert mask.sum() <= mask.size // 2000
+    target = rng.rand(*full.shape).astype(np.float32)
+    ct = cuda(keep[..., None])
+    loss = (((out - cuda(target)) * ct) ** 2).sum()
+    loss.backward()
+    with torch.no_grad():
+        guide = np_(models.HDRNetCurves._guide(cuda(full), params))
+        grid = np_(models.HDRNetCurves._coefficients(cuda(low), params))
+    ctn = 2.0 * (np_(out).astype(np.float64) - target) * keep[..., None] ** 2
+    sv = slice_f64.bilateral_slice_apply_grad(grid.reshape(16, 16, 16, 8, 12), guide, full, ctn, True)
+    want = coefficient_grads_f64(cuda(low), wts, sv.grid.reshape(16, 16, 16, 8, 3, 4))
+    gv = guide_f64.vjp(full, sv.guide, wn)
+    errs = {}
+
+    def rel(got, ref):
+        return float(np.abs(np.asarray(got, np.float64) - ref).max() / max(np.abs(ref).max(), 1e-30))
+
+    for k in C.variable_names(TRAIN):
+        errs[k.replace(C.P + "/", "")] = e = rel(np_(wts[k].grad), want[k])
+        assert e <= 1e-5, f"{k}: {e:.3e}"
+    for n in guide_f64.NAMES:
+        errs["guide/" + n] = e = rel(np_(wts[f"{G}/{n}"].grad), gv.dparams[n])
+        assert e <= 1e-5, f"{n}: {e:.3e}"
+    errs["fullres_input"] = e = rel(np_(tf.grad), sv.input + gv.dinput)
+    assert e <= 1e-5, f"fullres_input: {e:.3e}"
+    report("model with guide_grad 16x512^2", **errs)
+
+
+def test_forward_is_unchanged_without_guide_gradients():
+    """Under no_grad, and with the key but nothing in the guide requiring grad, the output is today's
+    (the fused kernel) bit for bit; with guide gradients the guide itself keeps its bits."""
+    params = dict(models.DEFAULT_PARAMS, net_input_size=64, spatial_bin=8)
+    wts = {k: v.detach() for k, v in model_weights(4).items()}
+    rng = np.random.RandomState(5)
+    low, full = cuda(rng.rand(2, 64, 64, 3)), cuda(rng.rand(2, 96, 160, 3))
+    with torch.no_grad():
+        today = models.HDRNetCurves.inference(low, full, dict(params, weights=wts))
+    with torch.no_grad():
+        got = models.HDRNetCurves.inference(low, full, dict(params, weights=wts, guide_grad=True))
+    assert torch.equal(got, today)
+    got = models.HDRNetCurves.inference(low, full, dict(params, weights=wts, guide_grad=True))
+    assert not got.requires_grad and torch.equal(got, today)
+    trained = dict(wts, **{f"{G}/ccm": wts[f"{G}/ccm"].clone().requires_grad_(True)})
+    with torch.no_grad():
+        g0 = models.HDRNetCurves._guide(full, dict(params, weights=wts))
+    g1 = models.HDRNetCurves._guide(full, dict(params, weights=trained, guide_grad=True))
+    assert g1.requires_grad and torch.equal(g1, g0)
+
+
+def test_teacher_with_another_guide_is_fitted_better_with_the_guide_trained():
+    """Teacher and student share the coefficient network; the teacher's guide is a non-identity
+    curve and ccm.  Adam at lr 1e-3 for 200 steps on one batch of 4 (64² network input, 128²
+    output), the coefficients trained in both runs, the guide only in one.  Measured on an H100:
+    the last-10-step mean loss was 2.16 with the guide fixed and 0.345 with it trained (a factor of
+    6.3, both from 7.73); the bar asks for a factor of 3."""
+    params = dict(models.DEFAULT_PARAMS, net_input_size=64, spatial_bin=8)
+    base = models.init_weights(params, seed=1)
+    rng = np.random.RandomState(8)
+    teacher = {k: torch.from_numpy(v).cuda() for k, v in base.items()}
+    teacher[f"{G}/ccm"] = cuda(np.array([[0.8, 0.2, 0.1], [0.3, 0.6, 0.1], [0.0, 0.3, 0.9]]))
+    teacher[f"{G}/slopes"] = cuda(np.abs(rng.randn(1, 1, 1, 3, 16)) * 0.15)
+    teacher[f"{G}/channel_mixing/weights"] = cuda(np.array([0.5, 0.3, 0.2]).reshape(1, 1, 3, 1))
+    full = cuda(rng.rand(4, 128, 128, 3))
+    low = cuda(np_(full)[:, ::2, ::2])
+    with torch.no_grad():
+        target = models.HDRNetCurves.inference(low, full, dict(params, weights=teacher))
+    final = {}
+    for train_guide in (False, True):
+        student = {k: torch.from_numpy(v).cuda().requires_grad_(k.startswith(C.P) or (train_guide and k.startswith(G)))
+                   for k, v in base.items()}
+        opt = torch.optim.Adam([v for v in student.values() if v.requires_grad], lr=1e-3)
+        p = dict(params, weights=student, guide_grad=train_guide)
+        losses = []
+        for _ in range(200):
+            opt.zero_grad()
+            loss = ((models.HDRNetCurves.inference(low, full, p) - target) ** 2).mean()
+            loss.backward()
+            opt.step()
+            losses.append(loss.item())
+        assert np.isfinite(losses).all()
+        final[train_guide] = float(np.mean(losses[-10:]))
+        report(f"teacher-guide fit train_guide={train_guide}", first=losses[0], last10=final[train_guide])
+    report("teacher-guide fit", ratio=final[False] / final[True])
+    assert final[True] * 3.0 <= final[False]

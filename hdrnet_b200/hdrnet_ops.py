@@ -21,6 +21,7 @@ with the reference's message; a failed launch raises ``HdrnetLibraryError`` (the
 from __future__ import annotations
 
 import ctypes
+import functools
 import threading
 
 import torch
@@ -82,6 +83,22 @@ def _workspace(dev: torch.device, nbytes: int) -> torch.Tensor:
     allocator hands a freed block back to the same stream only (stream-ordered reuse), so dropping
     the tensor right after the launch is safe."""
     return torch.empty((max(int(nbytes), 16) + 3) // 4, dtype=torch.float32, device=dev)
+
+
+@functools.lru_cache(maxsize=256)
+def _texture_form_runs(device_index: int, B: int, rows: int, W: int, gh: int, gw: int, gd: int) -> bool:
+    """Whether AUTO runs a texture-assisted form of the 3 -> 3 op on B x rows x W pixels when lent a
+    slab workspace (hdrnet_slice_apply_plan_ws answers): from 2 Mi pixels on, and only while the slab
+    rows fit one texture, 2^27 float4 texels (87,381 image rows of a 32x32x16 grid).  Past that AUTO
+    runs the TMA row kernel, and a lent workspace of over 2 GiB would go unused."""
+    if B * rows * W < (1 << 21) or W % 4:
+        return False
+    v = ctypes.c_int()
+    with torch.cuda.device(device_index):
+        rc = _lib.load().hdrnet_slice_apply_plan_ws(B, rows, W, gh, gw, gd, 3, 3, 1, 1, ctypes.byref(v),
+                                                    None, None, None)
+    _lib.check(rc, "slice-apply plan")
+    return v.value in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
 
 
 def _check_slice_args(grid, guide, grid_msg):
@@ -233,7 +250,8 @@ def bilateral_slice_apply(grid: torch.Tensor, guide: torch.Tensor, input: torch.
             ws_ptr, ws_bytes = 0, 0
             explicit_tex = int(variant) in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
             if (int(variant) == _lib.VARIANT_AUTO or explicit_tex) and n_in == 3 and n_out == 3 \
-                    and has_offset and W % 4 == 0 and (explicit_tex or B * H * W >= (1 << 21)):
+                    and has_offset and W % 4 == 0 and \
+                    (explicit_tex or _texture_form_runs(dev.index, B, H, W, gh, gw, gd)):
                 ws = _workspace(dev, lib.hdrnet_slice_apply_workspace_bytes(B, H, gw, gd))
                 ws_ptr, ws_bytes = ws.data_ptr(), ws.numel() * 4
             rc = lib.hdrnet_slice_apply_f32_ws(
@@ -311,7 +329,8 @@ def bilateral_slice_apply_rows(grid: torch.Tensor, guide: torch.Tensor, input: t
         ws_ptr, ws_bytes = 0, 0
         explicit_tex = int(variant) in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
         if (int(variant) == _lib.VARIANT_AUTO or explicit_tex) and n_in == 3 and n_out == 3 \
-                and has_offset and W % 4 == 0 and (explicit_tex or B * rows * W >= (1 << 21)):
+                and has_offset and W % 4 == 0 and \
+                (explicit_tex or _texture_form_runs(dev.index, B, rows, W, gh, gw, gd)):
             ws = _workspace(dev, lib.hdrnet_slice_apply_workspace_bytes(B, rows, gw, gd))
             ws_ptr, ws_bytes = ws.data_ptr(), ws.numel() * 4
         rc = lib.hdrnet_slice_apply_rows_f32_ws(

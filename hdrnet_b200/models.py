@@ -783,8 +783,8 @@ class HDRNetCurves(object):
             # workspace lent to the library (it never allocates): texture-assisted kernel for
             # large images, exactly as hdrnet_ops.bilateral_slice_apply does
             ws_ptr, ws_bytes = 0, 0
-            if B * H * W >= (1 << 21) and W % 4 == 0:
-                from .hdrnet_ops import _workspace
+            from .hdrnet_ops import _texture_form_runs, _workspace
+            if _texture_form_runs(fullres_input.device.index, B, H, W, gh, gw, gd):
                 ws = _workspace(fullres_input.device,
                                 lib.hdrnet_slice_apply_workspace_bytes(B, H, gw, gd))
                 ws_ptr, ws_bytes = ws.data_ptr(), ws.numel() * 4

@@ -102,8 +102,9 @@ def _shapes(grid, guide, inp, has_offset):
     return B, H, W, gh, gw, gd, gc, n_in, gc // J, J
 
 
-def _run(grid, guide, inp, ct, has_offset, want_grads):
-    """The one pass behind every entry point.  apply mode when ``inp`` is given."""
+def _run(grid, guide, inp, ct, has_offset, want_grads, y_off=0, height=None):
+    """The one pass behind every entry point.  apply mode when ``inp`` is given.  ``guide`` / ``inp``
+    hold image rows ``y_off ..`` of images ``height`` rows tall (default: the whole image)."""
     grid = np.asarray(grid, np.float64)
     guide = np.asarray(guide)
     inp = None if inp is None else np.asarray(inp, np.float64)
@@ -118,14 +119,18 @@ def _run(grid, guide, inp, ct, has_offset, want_grads):
         uv = np.zeros((B, H * W))
         uv_abs = np.zeros((B, H * W))
         iv = np.zeros((B, H * W, n_in)) if apply else None
-    (ys, wys) = _axis(H, gh)
+    if height is None:
+        height = H
+    if y_off < 0 or y_off + H > height:
+        raise ValueError(f"rows [{y_off}, {y_off + H}) do not fit an image of {height} rows")
+    (ys, wys) = _axis(height, gh)
     (xs, wxs) = _axis(W, gw)
     guide_f = guide.reshape(B, H * W)
     for b in range(B):
         gflat = grid[b].reshape(ncell, gc)
         for p0 in range(0, H * W, _CHUNK):
             p = np.arange(p0, min(p0 + _CHUNK, H * W))
-            y, x = p // W, p % W
+            y, x = p // W + y_off, p % W
             zc, zw, zwv, zdw = _depth(guide_f[b, p], gd)
             if apply:
                 ext = inp[b].reshape(H * W, n_in)[p]
@@ -178,9 +183,12 @@ def bilateral_slice(grid, guide) -> np.ndarray:
     return _run(grid, guide, None, None, False, False)
 
 
-def bilateral_slice_apply(grid, guide, inp, has_offset: bool) -> np.ndarray:
-    """-> [B,H,W,n_out], float64; grid channel c = i * (n_in + has_offset) + j."""
-    return _run(grid, guide, inp, None, has_offset, False)
+def bilateral_slice_apply(grid, guide, inp, has_offset: bool, y_off: int = 0, height=None) -> np.ndarray:
+    """-> [B,H,W,n_out], float64; grid channel c = i * (n_in + has_offset) + j.  With ``height``,
+    ``guide`` / ``inp`` are the row band ``y_off .. y_off + H - 1`` of images ``height`` rows tall
+    (what ``hdrnet_ops.bilateral_slice_apply_rows`` computes): a few rows of a large image cost
+    only their own pixels."""
+    return _run(grid, guide, inp, None, has_offset, False, y_off, height)
 
 
 def bilateral_slice_grad(grid, guide, ct) -> SliceVjps:
@@ -188,6 +196,7 @@ def bilateral_slice_grad(grid, guide, ct) -> SliceVjps:
     return _run(grid, guide, None, ct, False, True)
 
 
-def bilateral_slice_apply_grad(grid, guide, inp, ct, has_offset: bool) -> SliceVjps:
-    """VJPs of bilateral_slice_apply for the tangent ``ct`` [B,H,W,n_out]."""
-    return _run(grid, guide, inp, ct, has_offset, True)
+def bilateral_slice_apply_grad(grid, guide, inp, ct, has_offset: bool, y_off: int = 0, height=None) -> SliceVjps:
+    """VJPs of bilateral_slice_apply for the tangent ``ct`` [B,H,W,n_out].  ``y_off`` / ``height`` as in
+    bilateral_slice_apply; the grid VJP is then the band's pixels' share of it."""
+    return _run(grid, guide, inp, ct, has_offset, True, y_off, height)

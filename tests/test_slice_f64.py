@@ -66,6 +66,19 @@ def test_f64_apply_matches_port(oracle_port, case, guides):
     _check_apply(grid, guide, inp, ct, ho, oracle_port, f"{case} {guides}")
 
 
+@pytest.mark.parametrize("y_off, rows", [(0, 7), (13, 5), (33, 7), (39, 1)])
+def test_f64_apply_row_band_is_the_whole_image_rows(y_off, rows):
+    """A row band (y_off, height) is, value for value, those rows of the whole-image call: the large
+    extents tests hold a few rows of a large image to the reference at the cost of those rows."""
+    grid, guide, inp = rand_case(7, 2, 40, 23, 6, 5, 4, signed=True)
+    whole = slice_f64.bilateral_slice_apply(grid, guide, inp, True)
+    band = slice_f64.bilateral_slice_apply(grid, guide[:, y_off:y_off + rows], inp[:, y_off:y_off + rows], True,
+                                           y_off=y_off, height=40)
+    assert np.array_equal(band, whole[:, y_off:y_off + rows])
+    with pytest.raises(ValueError):
+        slice_f64.bilateral_slice_apply(grid, guide[:, :rows], inp[:, :rows], True, y_off=41 - rows, height=40)
+
+
 @pytest.mark.parametrize("case", SLICE_CASES, ids=str)
 def test_f64_slice_matches_port(oracle_port, case):
     B, H, W, gh, gw, gd, gc = case

@@ -18,7 +18,6 @@
 #include <algorithm>
 #include <atomic>
 #include <cstdint>
-#include <cstdlib>
 
 #include "hdrnet_b200.h"
 
@@ -844,12 +843,9 @@ static int conv_dispatch(const ConvArgs& a, bool pdl, cudaStream_t stream) {
   if (a.B == 0) return HDRNET_OK;
   {  // Tensor-core path (conv_wgmma.cu).  Each 128-pixel tile runs a fixed-latency chunk loop,
      // so it pays off once there are about as many tiles as SMs (H100, tools/conv_bench.py: about
-     // even with the CUDA-core kernels at 64 tiles, 1.8-3.7x faster at 128); HDRNET_CONV_TCGEN05=1
-     // / =0 forces it on / off.
-    const char* e = std::getenv("HDRNET_CONV_TCGEN05");   // per call: tests and smoke() flip it in-process
+     // even with the CUDA-core kernels at 64 tiles, 1.8-3.7x faster at 128).
     const long long tiles = (static_cast<long long>(a.B) * a.OH * a.OW + 127) / 128;
-    const bool want = e ? (e[0] == '1') : (tiles >= 96);
-    if (want) {
+    if (tiles >= 96) {
       const int rc = launch_conv_wgmma(a.in, a.w, a.bias, a.out, a.B, a.H, a.W, a.Cin, a.Cout, a.k, a.stride,
                                        a.relu, a.OH, a.OW, a.pad_t, a.pad_l, stream);
       if (rc != HDRNET_E_UNSUPPORTED) return rc;
@@ -880,8 +876,7 @@ static int conv_dispatch_pair(const ConvArgs& a, const ConvArgs& b, bool pdl, cu
     return ((px + 127) / 128) < 96 && patch_ok(c);
   };
   if (a.Cout == b.Cout && a.B > 0 && b.B > 0 && small(a) && small(b) &&
-      patch_slices(a.k * a.k * a.Cin) == patch_slices(b.k * b.k * b.Cin) &&
-      !std::getenv("HDRNET_CONV_TCGEN05")) {
+      patch_slices(a.k * a.k * a.Cin) == patch_slices(b.k * b.k * b.Cin)) {
     const auto tiles = [](const ConvArgs& c) {
       return (static_cast<long long>(c.B) * c.OH * c.OW + kPatchPx - 1) / kPatchPx;
     };

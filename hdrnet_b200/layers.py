@@ -100,7 +100,7 @@ def conv(inputs: torch.Tensor, num_outputs: int, kernel_size: int, stride: int =
     fused, post = _activation(activation_fn)
     with torch.cuda.device(inputs.device):
         if _differentiable(inputs, w, b):
-            out = models._ConvFn.apply(inputs, w, b, stride, fused, False)
+            out = models._ConvFn.apply(inputs, w, b, stride, fused)
         else:
             out = models._conv(inputs.contiguous(), (w, b), stride=stride, relu=fused)
     return out if post is None else post(out)

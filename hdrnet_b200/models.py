@@ -40,7 +40,6 @@ from __future__ import annotations
 
 import collections
 import ctypes
-import os
 import math
 
 import numpy as np
@@ -381,16 +380,11 @@ def pack_conv_weights(w: torch.Tensor):
     return packed
 
 
-def _use_packed_tc(tiles: int) -> bool:
-    """HDRNET_CONV_TCGEN05: '1' = tensor-core convs wherever weights were packed, '0' = never.
-    Default: from 64 tiles of 128 output pixels up.  Measured on an H100 (tools/conv_bench.py, the
-    network's conv shapes): at 16 tiles the CUDA-core kernels were 3-15 % faster, at 64 the two
-    were even, at 128 the packed tensor-core kernel was 1.7-5x faster."""
-    import os
-    flag = os.environ.get("HDRNET_CONV_TCGEN05")
-    if flag is not None:
-        return flag == "1"
-    return tiles >= 64
+# Layers given packed weights take the packed tensor-core form from this many tiles of 128 output
+# pixels up.  Measured on an H100 (tools/conv_bench.py, the network's conv shapes): at 16 tiles the
+# CUDA-core kernels were 3-15 % faster, at 64 the two were even, at 128 the packed tensor-core
+# kernel was 1.7-5x faster.
+PACKED_CONV_MIN_TILES = 64
 
 
 def _conv(x: torch.Tensor, wb, stride=1, relu=True) -> torch.Tensor:
@@ -403,7 +397,7 @@ def _conv(x: torch.Tensor, wb, stride=1, relu=True) -> torch.Tensor:
     oh, ow = -(-H // stride), -(-W // stride)
     out = torch.empty((B, oh, ow, cout), dtype=torch.float32, device=x.device)
     lib = _lib.load()
-    if packed is not None and _use_packed_tc((B * oh * ow + 127) // 128):
+    if packed is not None and (B * oh * ow + 127) // 128 >= PACKED_CONV_MIN_TILES:
         rc = lib.hdrnet_conv2d_nhwc_tc_f32(x.data_ptr(), packed.data_ptr(),
                                            0 if b is None else b.data_ptr(), out.data_ptr(), B, H,
                                            W, cin, cout, k, stride, int(relu),
@@ -447,21 +441,24 @@ def _ptr(t) -> int:
     return 0 if t is None else t.data_ptr()
 
 
+# Each layer Function's `run` is its forward alone, on the current device, for calls that want no
+# gradient: Function.apply costs host time on every layer, and a setup_context split would make
+# apply itself slower (it binds the arguments through inspect.signature on every call).
 class _ConvFn(torch.autograd.Function):
-    """One conv layer (hdrnet/layers.py:25-59, inference batch norm already folded): forward
-    hdrnet_conv2d_nhwc_f32 / its tensor-core form, backward hdrnet_conv2d_grad_f32."""
+    """One conv layer (hdrnet/layers.py:25-59, inference batch norm already folded): forward _conv
+    (given `packed`, pack_conv_weights of w, the packed tensor-core form from PACKED_CONV_MIN_TILES
+    up), backward hdrnet_conv2d_grad_f32."""
 
     @staticmethod
-    def forward(ctx, x, w, b, stride, relu, tc=True):
-        x, w = x.contiguous(), w.contiguous()
+    def run(x, w, b, stride, relu, packed=None):
         b = None if b is None else b.contiguous()
-        B, H, W, _ = x.shape
-        oh, ow = -(-H // stride), -(-W // stride)
-        # tc: the packed tensor-core form where _conv would take it (the model path; layers.conv
-        # never packs).  The variables change between optimizer steps, so they are packed per call.
-        packed = pack_conv_weights(w) if (tc and _use_packed_tc((B * oh * ow + 127) // 128)) else None
+        return _conv(x.contiguous(), (w.contiguous(), b, packed), stride=stride, relu=relu)
+
+    @staticmethod
+    def forward(ctx, x, w, b, stride, relu, packed=None):
+        x, w = x.contiguous(), w.contiguous()
         with torch.cuda.device(x.device):
-            out = _conv(x, (w, b, packed), stride=stride, relu=relu)
+            out = _ConvFn.run(x, w, b, stride, relu, packed)
         ctx.save_for_backward(x, w, out)
         ctx.stride, ctx.relu, ctx.has_bias = stride, bool(relu), b is not None
         return out
@@ -494,11 +491,15 @@ class _FcFn(torch.autograd.Function):
     hdrnet_fc_grad_f32."""
 
     @staticmethod
+    def run(x, w, b, relu):
+        b = None if b is None else b.contiguous()
+        return _fc(x.contiguous(), (w.contiguous(), b), relu=relu)
+
+    @staticmethod
     def forward(ctx, x, w, b, relu):
         x, w = x.contiguous(), w.contiguous()
-        b = None if b is None else b.contiguous()
         with torch.cuda.device(x.device):
-            out = _fc(x, (w, b), relu=relu)
+            out = _FcFn.run(x, w, b, relu)
         ctx.save_for_backward(x, w, out)
         ctx.relu, ctx.has_bias = bool(relu), b is not None
         return out
@@ -531,16 +532,22 @@ class _FusePredictFn(torch.autograd.Function):
     saved local and global)."""
 
     @staticmethod
-    def forward(ctx, local, glob, w, b, gd, n_out, n_in):
+    def run(local, glob, w, b, gd, n_out, n_in):
         local, glob, w = local.contiguous(), glob.contiguous(), w.contiguous()
         b = None if b is None else b.contiguous()
         bs, gh, gw, C = local.shape
         grid = torch.empty((bs, gh, gw, gd, n_out, n_in), dtype=torch.float32, device=local.device)
-        with torch.cuda.device(local.device):
-            rc = _lib.load().hdrnet_fuse_predict_f32(
-                local.data_ptr(), glob.data_ptr(), w.data_ptr(), _ptr(b), grid.data_ptr(), bs, gh, gw,
-                C, gd, n_out, n_in, _stream(local.device))
+        rc = _lib.load().hdrnet_fuse_predict_f32(
+            local.data_ptr(), glob.data_ptr(), w.data_ptr(), _ptr(b), grid.data_ptr(), bs, gh, gw,
+            C, gd, n_out, n_in, _stream(local.device))
         _lib.check(rc, "fuse_predict")
+        return grid
+
+    @staticmethod
+    def forward(ctx, local, glob, w, b, gd, n_out, n_in):
+        local, glob, w = local.contiguous(), glob.contiguous(), w.contiguous()
+        with torch.cuda.device(local.device):
+            grid = _FusePredictFn.run(local, glob, w, b, gd, n_out, n_in)
         ctx.save_for_backward(local, glob, w)
         ctx.dims, ctx.has_bias = (gd, n_out, n_in), b is not None
         return grid
@@ -811,65 +818,46 @@ class HDRNetCurves(object):
         _refuse_batch_norm(_weights_or_none(params), params)
         x = _check_input(input_tensor, "lowres_input")
         prep = _prepare(_resolve_weights(params), params, x.device, cls._nn_guide)
-        L = prep.layers
-        gd = params["luma_bins"]
-        p = "inference/coefficients"
-        n_ds = int(np.log2(params["net_input_size"] / params["spatial_bin"]))
-        bs = x.shape[0]
-        if torch.is_grad_enabled() and (x.requires_grad or any(
-                _requires_grad(t) for wb in L.values() for t in wb[:2])):
-            return cls._coefficients_autograd(x, L, gd, n_ds)
+        grad = torch.is_grad_enabled() and (x.requires_grad or any(
+            _requires_grad(t) for wb in prep.layers.values() for t in wb[:2]))
         # small batches: the whole network behind one library call (launch chain, csrc/cnn.cu)
-        if bs <= CHAIN_CNN_MAX_BATCH and os.environ.get("HDRNET_CONV_TCGEN05") != "1":
-            grid = cls._coefficients_chain(x, prep, params, n_ds)
+        if not grad and x.shape[0] <= CHAIN_CNN_MAX_BATCH:
+            grid = cls._coefficients_chain(x, prep, params)
             if grid is not None:
                 return grid
-        with torch.cuda.device(x.device):
-            for i in range(n_ds):                                   # splat, :69-82
-                x = _conv(x, L[f"{p}/splat/conv{i + 1}"], stride=2)
-            splat = x
-            g = _conv(splat, L[f"{p}/global/conv1"], stride=2)      # global, :86-105
-            g = _conv(g, L[f"{p}/global/conv2"], stride=2)
-            g = g.reshape(bs, -1)                                   # NHWC flatten, :94-95
-            g = _fc(g, L[f"{p}/global/fc1"])
-            g = _fc(g, L[f"{p}/global/fc2"])
-            g = _fc(g, L[f"{p}/global/fc3"], relu=False)
-            loc = _conv(splat, L[f"{p}/local/conv1"])               # local, :109-118
-            loc = _conv(loc, L[f"{p}/local/conv2"], relu=False)
-            wp, bp = L[f"{p}/prediction/conv1"][:2]
-            _, gh, gw, C = loc.shape
-            grid = torch.empty((bs, gh, gw, gd, cls.n_out(), cls.n_in()), dtype=torch.float32,
-                               device=x.device)
-            rc = _lib.load().hdrnet_fuse_predict_f32(           # fusion+prediction+unroll, :122-139
-                loc.data_ptr(), g.data_ptr(), wp.data_ptr(), 0 if bp is None else bp.data_ptr(),
-                grid.data_ptr(), bs, gh, gw, C, gd, cls.n_out(), cls.n_in(),
-                torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(rc, "fuse_predict")
-        return grid
+        n_ds = int(np.log2(params["net_input_size"] / params["spatial_bin"]))
+        return cls._coefficients_layers(x, prep.layers, params["luma_bins"], n_ds, grad)
 
     @classmethod
-    def _coefficients_autograd(cls, x, L, gd, n_ds):
-        """The per-layer path above with every layer an autograd Function: the same kernels in the
-        same order (so the same values, bitwise), and a backward through csrc/cnn_grad.cu."""
+    def _coefficients_layers(cls, x, L, gd, n_ds, grad):
+        """Layer by layer over the prepared weights: with `grad` every layer an autograd Function
+        (backward through csrc/cnn_grad.cu), else only its forward (`run`)."""
+        conv_fn, fc_fn, fuse_fn = (f.apply if grad else f.run for f in (_ConvFn, _FcFn, _FusePredictFn))
         p = "inference/coefficients"
         bs = x.shape[0]
+
+        def conv(x, scope, stride, relu=True):
+            w, b, packed = L[f"{p}/{scope}"]
+            return conv_fn(x, w, b, stride, relu, packed)
+
         with torch.cuda.device(x.device):
-            for i in range(n_ds):
-                x = _ConvFn.apply(x, *L[f"{p}/splat/conv{i + 1}"][:2], 2, True)
+            for i in range(n_ds):                                   # splat, :69-82
+                x = conv(x, f"splat/conv{i + 1}", 2)
             splat = x
-            g = _ConvFn.apply(splat, *L[f"{p}/global/conv1"][:2], 2, True)
-            g = _ConvFn.apply(g, *L[f"{p}/global/conv2"][:2], 2, True)
-            g = g.reshape(bs, -1)
-            g = _FcFn.apply(g, *L[f"{p}/global/fc1"][:2], True)
-            g = _FcFn.apply(g, *L[f"{p}/global/fc2"][:2], True)
-            g = _FcFn.apply(g, *L[f"{p}/global/fc3"][:2], False)
-            loc = _ConvFn.apply(splat, *L[f"{p}/local/conv1"][:2], 1, True)
-            loc = _ConvFn.apply(loc, *L[f"{p}/local/conv2"][:2], 1, False)
+            g = conv(splat, "global/conv1", 2)                      # global, :86-105
+            g = conv(g, "global/conv2", 2)
+            g = g.reshape(bs, -1)                                   # NHWC flatten, :94-95
+            g = fc_fn(g, *L[f"{p}/global/fc1"][:2], True)
+            g = fc_fn(g, *L[f"{p}/global/fc2"][:2], True)
+            g = fc_fn(g, *L[f"{p}/global/fc3"][:2], False)
+            loc = conv(splat, "local/conv1", 1)                     # local, :109-118
+            loc = conv(loc, "local/conv2", 1, relu=False)
             wp, bp = L[f"{p}/prediction/conv1"][:2]                 # HWIO [1, 1, C, O] -> [C, O]
-            return _FusePredictFn.apply(loc, g, wp.reshape(wp.shape[-2:]), bp, gd, cls.n_out(), cls.n_in())
+            # fusion + prediction + unroll, :122-139
+            return fuse_fn(loc, g, wp.reshape(wp.shape[-2:]), bp, gd, cls.n_out(), cls.n_in())
 
     @classmethod
-    def _coefficients_chain(cls, x, prep, params, n_ds):
+    def _coefficients_chain(cls, x, prep, params):
         """One library call for all layers; None when the library does not take the shape."""
         lib = _lib.load()
         bs, S = x.shape[0], x.shape[1]
@@ -877,10 +865,7 @@ class HDRNetCurves(object):
         nbytes = lib.hdrnet_coefficients_scratch_bytes(bs, S, sb, gd, cm, cls.n_out(), cls.n_in())
         if nbytes == 0 or x.shape[2] != S:
             return None
-        p = "inference/coefficients"
-        order = [f"{p}/splat/conv{i + 1}" for i in range(n_ds)] + \
-                [f"{p}/global/conv1", f"{p}/global/conv2", f"{p}/global/fc1", f"{p}/global/fc2",
-                 f"{p}/global/fc3", f"{p}/local/conv1", f"{p}/local/conv2", f"{p}/prediction/conv1"]
+        order = [scope for scope, _, _ in _coefficient_specs(params)]
         ptrs = getattr(prep, "_pc_ptrs", None)
         if ptrs is None:     # host arrays of device pointers, built once per prepared model
             n = len(order)

@@ -274,8 +274,8 @@ HDRNET_API int hdrnet_conv2d_nhwc_f32(const float* in, const float* w, const flo
  * in the MMA's shared-memory layout (hdrnet_conv2d_tc_packed_bytes() bytes, 16-byte aligned device
  * memory owned by the caller: HDRNET_E_UNSUPPORTED otherwise); the layer call then needs
  * Cin % 4 == 0, Cout % 16 == 0, 16 <= Cout <= 128.
- * hdrnet_conv2d_nhwc_f32 also reaches an unpacked tensor-core kernel on its own when the layer
- * has >= 96 tiles of 128 pixels (HDRNET_CONV_TCGEN05=0/1 overrides).
+ * hdrnet_conv2d_nhwc_f32 runs an unpacked tensor-core kernel on its own when the layer has
+ * >= 96 tiles of 128 output pixels and its shape suits that kernel.
  */
 HDRNET_API size_t hdrnet_conv2d_tc_packed_bytes(int k, int Cin, int Cout);
 HDRNET_API int hdrnet_conv2d_tc_pack_f32(const float* w, float* packed, int k, int Cin, int Cout,

@@ -386,7 +386,6 @@ def test_coefficients_with_flat_buffer_weights(B, per_layer, monkeypatch):
     convs with scalar weight staging and the plain fc kernel."""
     wts, low, want = network_case(B)
     _, views, _ = flat_weights(wts, TRAIN)
-    monkeypatch.delenv("HDRNET_CONV_TCGEN05", raising=False)
     if per_layer:
         monkeypatch.setattr(models, "CHAIN_CNN_MAX_BATCH", 0)
     with torch.no_grad():

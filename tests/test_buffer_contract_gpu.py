@@ -661,8 +661,7 @@ CONV_CASES = {
 
 @gpu
 @pytest.mark.parametrize("name", list(CONV_CASES))
-def test_conv(name, monkeypatch):
-    monkeypatch.delenv("HDRNET_CONV_TCGEN05", raising=False)
+def test_conv(name):
     B, H, W, cin, cout, k, s, packed = CONV_CASES[name]
     rng = np.random.RandomState(180 + cout)
     x = rng.randn(B, H, W, cin).astype(np.float32)
@@ -730,10 +729,9 @@ NET = dict(M.DEFAULT_PARAMS, net_input_size=128, spatial_bin=16)
 
 @gpu
 @pytest.mark.parametrize("B", [1, 4, 16, 17])
-def test_coefficients(B, monkeypatch):
+def test_coefficients(B):
     """B <= 16: the whole network behind one call, its scratch allocated at exactly
     hdrnet_coefficients_scratch_bytes; B = 17: layer by layer (tensor-core convs on packed weights)."""
-    monkeypatch.delenv("HDRNET_CONV_TCGEN05", raising=False)
     assert models.CHAIN_CNN_MAX_BATCH == 16
     wts = M.make_weights(NET, seed=200)
     low = np.random.RandomState(201 + B).rand(B, 128, 128, 3).astype(np.float32)

@@ -312,13 +312,22 @@ def test_nothing_stale_and_inference_equals_the_differentiable_forward(model, mo
     wts = tensor_weights(params, model_name=model.__name__)
     _, low, full = small_setup(B=3)
     monkeypatch.setattr(models, "CHAIN_CNN_MAX_BATCH", 0)        # the per-layer inference path
-    for tc in ("0", "1"):                                         # CUDA-core and tensor-core convs
-        monkeypatch.setenv("HDRNET_CONV_TCGEN05", tc)
-        grid = model._coefficients(low, dict(params, weights=wts))
+    # output pixels per image of every conv layer (SAME padding halves the extent at stride 2)
+    S, n_ds = params["net_input_size"], int(np.log2(params["net_input_size"] / params["spatial_bin"]))
+    side = {f"{P}/splat/conv{i + 1}": S >> (i + 1) for i in range(n_ds)}
+    side.update({f"{P}/global/conv1": S >> (n_ds + 1), f"{P}/global/conv2": S >> (n_ds + 2),
+                 f"{P}/local/conv1": S >> n_ds, f"{P}/local/conv2": S >> n_ds})
+    px = {s: n * n for s, n in side.items()}
+    packable = [s for s in px if models.pack_conv_weights(wts[s + "/weights"].detach()) is not None]
+    packed_px = models.PACKED_CONV_MIN_TILES * 128                # tiles of 128 output pixels
+    assert 3 * max(px.values()) < packed_px                       # batch 3: CUDA-core convs only
+    packed_batch = -(-packed_px // max(px[s] for s in packable))  # the largest packable layer runs packed
+    for B in (3, packed_batch):
+        low_b = small_setup(B=B)[1]
+        grid = model._coefficients(low_b, dict(params, weights=wts))
         assert grid.requires_grad
         with torch.no_grad():
-            assert torch.equal(model._coefficients(low, dict(params, weights=wts)), grid)
-    monkeypatch.delenv("HDRNET_CONV_TCGEN05")
+            assert torch.equal(model._coefficients(low_b, dict(params, weights=wts)), grid)
     with torch.no_grad():
         before = model.inference(low, full, dict(params, weights=wts)).clone()
     opt = torch.optim.Adam([v for v in wts.values() if v.requires_grad], lr=1e-2)

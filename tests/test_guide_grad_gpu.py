@@ -259,9 +259,10 @@ def coefficient_grads_f64(low, wts, dgrid):
          for s, _, _ in models._coefficient_specs(TRAIN)}
     acts = {}
 
-    def conv(s, x, stride, relu):
-        acts[s] = (x, models._ConvFn.apply(x, *L[s], stride, relu), stride, relu)
-        return acts[s][1]
+    def conv(s, x, stride, relu):       # the packed weights the model's forward used
+        out = models._ConvFn.apply(x, *L[s], stride, relu, models.pack_conv_weights(L[s][0]))
+        acts[s] = (x, out, stride, relu)
+        return out
 
     def fc(s, x, relu):
         acts[s] = (x, models._FcFn.apply(x, *L[s], relu), None, relu)

@@ -192,7 +192,6 @@ def test_coefficients_chain_and_per_layer_paths_agree(name, B, monkeypatch):
     lib = _lib.load()
     assert lib.hdrnet_coefficients_scratch_bytes(B, S, p["spatial_bin"], p["luma_bins"], p["channel_multiplier"],
                                                  cls.n_out(), cls.n_in()) > 0
-    monkeypatch.delenv("HDRNET_CONV_TCGEN05", raising=False)
     monkeypatch.setattr(models, "CHAIN_CNN_MAX_BATCH", 64)
     one = cls._coefficients(cuda(low), dict(p, weights=wts)).cpu().numpy()
     monkeypatch.setattr(models, "CHAIN_CNN_MAX_BATCH", 0)
@@ -222,7 +221,6 @@ def test_coefficient_chain_argument_checks_and_odd_channel_counts(monkeypatch):
     p = dict(M.DEFAULT_PARAMS, luma_bins=6, net_input_size=64, spatial_bin=16)
     wts = M.make_weights(p, seed=1)
     low = np.random.RandomState(2).rand(1, 64, 64, 3).astype(np.float32)
-    monkeypatch.delenv("HDRNET_CONV_TCGEN05", raising=False)
     for mb in (64, 0):
         monkeypatch.setattr(models, "CHAIN_CNN_MAX_BATCH", mb)
         got = models.HDRNetCurves._coefficients(cuda(low), dict(p, weights=wts)).cpu().numpy()
@@ -338,12 +336,13 @@ def test_run_py_identity_sample_plumbing(tmp_path):
     assert np.abs(out8.astype(int) - ref8.astype(int)).max() <= 1
 
 
-# ---- tensor-core (wgmma, 3xTF32) form of the conv layers (named after the HDRNET_CONV_TCGEN05 knob) ----
-@pytest.fixture
-def tcgen05_convs(monkeypatch):
-    monkeypatch.setenv("HDRNET_CONV_TCGEN05", "1")
-    monkeypatch.setattr(models, "CHAIN_CNN_MAX_BATCH", 0)    # per-layer calls from Python, not the chain
-    yield
+# ---- tensor-core (wgmma, 3xTF32) forms of the conv layers --------------------------------------
+def conv_case(rng, B, H, W, cin, cout, k, stride, relu, bias):
+    x = rng.randn(B, H, W, cin).astype(np.float32)
+    w = (rng.randn(k, k, cin, cout) / np.sqrt(k * k * cin)).astype(np.float32)
+    b = rng.randn(cout).astype(np.float32) if bias else None
+    ref = M.conv2d_same(x, w, stride) + (0 if b is None else b)
+    return x, w, b, (np.maximum(ref, 0) if relu else ref).astype(np.float32)
 
 
 @pytest.mark.gpu
@@ -351,39 +350,48 @@ def tcgen05_convs(monkeypatch):
     (8, 16, 16, 64, 64, 3, 1, True, True),     # local conv1 (models.py:109-113)
     (1, 16, 16, 64, 64, 3, 1, False, False),   # local conv2 at batch 1: 2 tiles
     (2, 32, 32, 32, 64, 3, 2, True, True),     # splat conv4, stride 2, SAME pad 0/1
+    (1, 16, 16, 64, 64, 3, 2, True, True),     # global conv1: half a tile
+    (1, 8, 8, 64, 64, 3, 2, True, True),       # global conv2: 16 px
     (3, 16, 16, 64, 96, 1, 1, False, True),    # 1x1 prediction, N = 96
     (1, 9, 7, 8, 16, 3, 1, True, True),        # ragged tile (63 px), K = 72 (partial last chunk)
     (1, 16, 16, 64, 192, 3, 1, True, True),    # Cout > 128: two launches over columns 0-127, 128-191
     (2, 12, 12, 32, 144, 3, 2, False, True),   # Cout = 128 + 16, stride 2
 ])
-def test_conv2d_tcgen05_matches_oracle(tcgen05_convs, B, H, W, cin, cout, k, stride, relu, bias):
+def test_conv2d_wgmma_matches_oracle(B, H, W, cin, cout, k, stride, relu, bias):
     """3xTF32 on the tensor cores keeps float32-grade accuracy: 1e-5 of the tensor's range (a plain
-    TF32 product would be ~1e-3)."""
+    TF32 product would be ~1e-3).  The packed form (pre-packed hi/lo weight tiles, 3-stage ring, one
+    TMA copy per chunk) through its entry point at the case's own shape; the unpacked form, which
+    hdrnet_conv2d_nhwc_f32 takes from 96 tiles of 128 output pixels, at the batch that reaches them."""
+    lib = _lib.load()
     rng = np.random.RandomState(11)
-    x = rng.randn(B, H, W, cin).astype(np.float32)
-    w = (rng.randn(k, k, cin, cout) / np.sqrt(k * k * cin)).astype(np.float32)
-    b = rng.randn(cout).astype(np.float32) if bias else None
-    ref = M.conv2d_same(x, w, stride) + (0 if b is None else b)
-    if relu:
-        ref = np.maximum(ref, 0)
-    got = models._conv(cuda(x), (cuda(w), None if b is None else cuda(b)), stride=stride, relu=relu)
-    torch.cuda.synchronize()
-    assert_parity(got.cpu().numpy(), ref.astype(np.float32), rtol=1e-5)
-    # pipelined kernel with pre-packed hi/lo weight tiles (3-stage ring, one TMA copy per chunk)
-    wd = cuda(w)
-    packed = models.pack_conv_weights(wd)
+    oh, ow = -(-H // stride), -(-W // stride)
     if cout <= 128:
+        x, w, b, ref = conv_case(rng, B, H, W, cin, cout, k, stride, relu, bias)
+        wd, bd, xd = cuda(w), None if b is None else cuda(b), cuda(x)
+        packed = models.pack_conv_weights(wd)
         assert packed is not None
-        got2 = models._conv(cuda(x), (wd, None if b is None else cuda(b), packed), stride=stride, relu=relu)
-        torch.cuda.synchronize()
-        assert_parity(got2.cpu().numpy(), ref.astype(np.float32), rtol=1e-5, what="packed/pipelined")
+        out = torch.empty((B, oh, ow, cout), device="cuda")
+        _lib.check(lib.hdrnet_conv2d_nhwc_tc_f32(xd.data_ptr(), packed.data_ptr(), 0 if bd is None else bd.data_ptr(),
+                                                 out.data_ptr(), B, H, W, cin, cout, k, stride, int(relu),
+                                                 torch.cuda.current_stream().cuda_stream), "conv2d (packed)")
+        assert_parity(out.cpu().numpy(), ref, rtol=1e-5, what="packed")
+    nb = max(B, -(-96 * 128 // (oh * ow)))
+    if (B * oh * ow) % 128 and not (nb * oh * ow) % 128:
+        nb += 1                                                      # a ragged last tile stays ragged
+    x, w, b, ref = conv_case(rng, nb, H, W, cin, cout, k, stride, relu, bias)
+    got = models._conv(cuda(x), (cuda(w), None if b is None else cuda(b)), stride=stride, relu=relu)
+    assert_parity(got.cpu().numpy(), ref, rtol=1e-5, what=f"unpacked at batch {nb}")
 
 
 @pytest.mark.gpu
-def test_coefficients_with_tcgen05_convs(tcgen05_convs):
+def test_coefficients_with_wgmma_convs():
+    """Layer by layer at batch 32: every packable layer of the default network but the two global
+    convs (test_conv2d_wgmma_matches_oracle has their shapes) has >= 64 tiles, so runs packed."""
+    B = 32
+    assert B > models.CHAIN_CNN_MAX_BATCH
     p = PARAM_SETS["default"]
     wts = M.make_weights(p, seed=3)
-    low = np.random.RandomState(4).rand(2, 256, 256, 3).astype(np.float32)
+    low = np.random.RandomState(4).rand(B, 256, 256, 3).astype(np.float32)
     ref = M.coefficients(low, wts, p)
     got = models.HDRNetCurves._coefficients(cuda(low), dict(p, weights=wts)).cpu().numpy()
     assert_parity(got, ref, rtol=5e-5, what="coefficients via tensor-core convs")

@@ -16,7 +16,7 @@ def t(fn, iters=50):
     return a.elapsed_time(b) / iters * 1e3
 
 
-for B in (1, 2, 4, 8, 16, 64):
+for B in (1, 2, 4, 8, 16, 32, 64):
     low = torch.rand(B, 256, 256, 3, device="cuda")
     res = {}
     for label, mb in (("chain", 64), ("per-layer", 0)):

@@ -58,31 +58,28 @@ def timed(fn, steps, warmup, reps):
 
 
 def layer_inputs(low, L, gd):
-    """Each layer's (Function, inputs, extra args) from one real forward."""
+    """Each layer's (Function, inputs, (weights, bias), extra args) from one real forward; the convs
+    get the model's packed weights."""
     out, x = [], low
     n_ds = sum(1 for k in L if "/splat/" in k)
+
+    def conv(s, x, stride, relu):
+        w, b, packed = L[s]
+        out.append((s, models._ConvFn, x, (w, b), (stride, relu, packed)))
+        return models._ConvFn.apply(x, w, b, stride, relu, packed)
+
     with torch.no_grad():
         for i in range(n_ds):
-            s = f"{P}/splat/conv{i + 1}"
-            out.append((s, models._ConvFn, x, L[s], (2, True)))
-            x = models._ConvFn.apply(x, *L[s], 2, True)
+            x = conv(f"{P}/splat/conv{i + 1}", x, 2, True)
         splat = x
-        s = f"{P}/global/conv1"
-        out.append((s, models._ConvFn, splat, L[s], (2, True)))
-        g = models._ConvFn.apply(splat, *L[s], 2, True)
-        s = f"{P}/global/conv2"
-        out.append((s, models._ConvFn, g, L[s], (2, True)))
-        g = models._ConvFn.apply(g, *L[s], 2, True).reshape(low.shape[0], -1)
+        g = conv(f"{P}/global/conv1", splat, 2, True)
+        g = conv(f"{P}/global/conv2", g, 2, True).reshape(low.shape[0], -1)
         for name, relu in (("fc1", True), ("fc2", True), ("fc3", False)):
             s = f"{P}/global/{name}"
-            out.append((s, models._FcFn, g, L[s], (relu,)))
-            g = models._FcFn.apply(g, *L[s], relu)
-        s = f"{P}/local/conv1"
-        out.append((s, models._ConvFn, splat, L[s], (1, True)))
-        loc = models._ConvFn.apply(splat, *L[s], 1, True)
-        s = f"{P}/local/conv2"
-        out.append((s, models._ConvFn, loc, L[s], (1, False)))
-        loc = models._ConvFn.apply(loc, *L[s], 1, False)
+            out.append((s, models._FcFn, g, L[s][:2], (relu,)))
+            g = models._FcFn.apply(g, *L[s][:2], relu)
+        loc = conv(f"{P}/local/conv1", splat, 1, True)
+        loc = conv(f"{P}/local/conv2", loc, 1, False)
     s = f"{P}/prediction/conv1"
     out.append((s, "fuse", (loc, g), L[s], (gd, 3, 4)))
     return out
@@ -160,8 +157,9 @@ def main():
                                    a.steps, a.warmup, a.reps)
 
     # every coefficient layer's VJP alone
-    L = {s: (wts[s + "/weights"] if "/prediction/" not in s else wts[s + "/weights"][0, 0],
-             wts.get(s + "/biases")) for s in (x[0] for x in models._coefficient_specs(params))}
+    # the model's prepared layers: the variables themselves, and the convs' packed weights
+    L = {s: (wb[0][0, 0], wb[1]) if "/prediction/" in s else wb
+         for s, wb in models._prepare(wts, params, low.device, False).layers.items()}
     layers = {}
     for scope, fn, x, wb, extra in layer_inputs(low, L, gd):
         if fn == "fuse":

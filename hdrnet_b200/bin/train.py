@@ -8,8 +8,11 @@ arguments, flags and defaults (train.py:188-244):
         [--max_steps N] [--seed S] [--[no]train_guide]
 
 ``data_dir`` holds ``filelist.txt`` and the ``input/`` and ``output/`` folders (or is that
-``filelist.txt``); hdrnet_b200/data_pipeline.py keeps the decoded pairs on the device and builds
-each batch in one kernel.  Each step runs ``inference`` with the coefficient-network variables
+``filelist.txt``); hdrnet_b200/data_pipeline.py decodes the pairs once and builds each batch in one
+kernel.  When the decoded pairs fit in the free device memory (less 2 GiB kept for the step) they
+are uploaded once and each batch is gathered on the device; otherwise they stay on the host, and
+each batch's crop windows are streamed to the device one to two steps ahead, with the same batches.
+``--data_threads`` threads decode the files and, when streaming, pack the windows.  Each step runs ``inference`` with the coefficient-network variables
 requiring grad, ``metrics.l2_loss`` and the per-image-mean ``metrics.psnr``, the backward and
 ``torch.optim.Adam(learning_rate)``.  An exponential moving average (0.99, zero-debiased as TF's
 averages of tensors are) of loss and PSNR is logged every ``--log_interval`` seconds, and the
@@ -50,6 +53,7 @@ Deliberate differences from the reference:
   step size.  With eps = 1e-8 the two differ only while sqrt(v) is of the order of eps.
 * No queue runners, summaries or TF event files: batches are built on the device when needed and
   the scalars go to ``train_log.jsonl``.  The random streams are not TF's (data_pipeline.py).
+* The decoded dataset must fit in host memory: every pair is decoded once at start-up.
 """
 from __future__ import annotations
 
@@ -101,7 +105,8 @@ def build_parser() -> argparse.ArgumentParser:
 
     data_grp = parser.add_argument_group("data pipeline")
     data_grp.add_argument("--batch_size", default=16, type=int, help="size of a batch for each gradient update.")
-    data_grp.add_argument("--data_threads", default=2, type=int, help="number of threads that decode the images at start-up.")
+    data_grp.add_argument("--data_threads", default=2, type=int,
+                          help="number of threads that decode the images at start-up (and pack streamed batches).")
     data_grp.add_argument("--rotate", dest="rotate", action="store_true", help="rotate data augmentation.")
     data_grp.add_argument("--norotate", dest="rotate", action="store_false")
     data_grp.add_argument("--flipud", dest="flipud", action="store_true", help="flip up/down data augmentation.")
@@ -305,6 +310,12 @@ class Trainer:
         with open(os.path.join(self.args.checkpoint_dir, "train_log.jsonl"), "a") as f:
             f.write(json.dumps(rec) + "\n")
 
+    def close(self):
+        """Stop the data pipelines' threads (those of a streamed tier)."""
+        for data in (self.train_data, self.eval_data):
+            if data is not None:
+                data.close()
+
     def run(self):
         a = self.args
         t0 = time.time()
@@ -337,6 +348,8 @@ class Trainer:
                     last_ckpt = time.time()
         except KeyboardInterrupt:
             log.info("interrupted at step %d", self.step)
+        finally:
+            self.close()
         log.info("Training complete, saving chkpt %s", os.path.join(a.checkpoint_dir, "on_stop.ckpt"))
         return self.save("on_stop.ckpt")
 

@@ -1,4 +1,4 @@
-"""Training data from image pairs, kept on the device: the reference's ``ImageFilesDataPipeline``
+"""Training data from image pairs, batched on the device: the reference's ``ImageFilesDataPipeline``
 (hdrnet/data_pipeline.py:126-240).
 
 Layout (data_pipeline.py:174-200): ``<data_dir>/filelist.txt`` names one file per line; the pair is
@@ -6,11 +6,21 @@ Layout (data_pipeline.py:174-200): ``<data_dir>/filelist.txt`` names one file pe
 ``filelist.txt`` in it (the reference's CLI is given the latter).
 
 At start-up every pair is decoded on ``nthreads`` host threads (``cv2.imread(IMREAD_UNCHANGED)``;
-alpha dropped, BGR -> RGB, grey replicated to 3 channels, as bin/run.py decodes) and uploaded once,
-in its storage format (uint8, uint16 or float32, chosen per file), into one device buffer.  Each
-batch is then ONE kernel (``hdrnet_train_batch_f32``, csrc/train_batch.cu) that gathers the flipped,
-rotated and cropped full-resolution input and target and the nearest-neighbour network input
-straight from that cache; the host only draws random numbers.
+alpha dropped, BGR -> RGB, grey replicated to 3 channels, as bin/run.py decodes) and kept in its
+storage format (uint8, uint16 or float32, chosen per file).  Each batch is ONE kernel
+(``hdrnet_train_batch_f32``, csrc/train_batch.cu) that gathers the flipped, rotated and cropped
+full-resolution input and target and the nearest-neighbour network input.  Where its sources live
+is chosen at start-up from the free device memory (``device_budget``):
+
+* Device tier, when the dataset fits beside ``memory_margin``: every pair is uploaded once into one
+  device buffer and the kernel reads the crops straight from it; the host only draws random numbers.
+* Streamed tier, otherwise: the decoded pairs stay on the host.  A crop reads only its
+  ``source_window``, so host threads copy each sample's input and target windows into one of two
+  pinned staging slots, one host-to-device copy per batch moves the slot to one of two device slots
+  on a copy stream, and the kernel reads the windows there.  Batches ``step + 1, step + 2`` are
+  built ahead while ``step`` trains; the batches are bitwise those of the device tier.
+
+Only when even the two device staging slots do not fit is ``MemoryError`` raised.
 
 Semantics are ``_augment_data`` (data_pipeline.py:126-171): flip left-right, flip up-down (each
 with p = 1/2), rot90 by k uniform in 0..3 (counter-clockwise), then a uniform random crop of
@@ -28,7 +38,7 @@ Deliberate differences:
   (data_pipeline.py:166).  They are equal at the default.
 * Each file keeps its own pixel format; the reference decides from the first file of each folder.
 * No queue runners: a batch is ready when its kernel has run.
-* The whole dataset must fit in device memory; streaming from the host is not implemented.
+* The whole dataset must fit in host memory: it is decoded once at start-up, not on demand.
 """
 from __future__ import annotations
 
@@ -37,6 +47,8 @@ import ctypes
 import functools
 import logging
 import os
+import threading
+import time
 from typing import NamedTuple
 
 import numpy as np
@@ -174,6 +186,36 @@ class Sampler:
         return out
 
 
+def source_window(H: int, W: int, draw: Draw, oh: int, ow: int):
+    """``(y0, x0, h, w)``: the rectangle of the un-augmented H x W source that ``draw``'s oh x ow crop
+    reads (h x w = oh x ow, or ow x oh when ``rot90`` is odd).
+
+    The crop maps onto the source as ``source_pixel`` in csrc/train_batch.cu does: rotation on the
+    flipped source.  Cut out as an image of its own, the window gives the same crop (and so the same
+    nearest-neighbour network input) under the same flips and rotation with the crop origin at
+    (0, 0)."""
+    cy, cx, k = int(draw.crop_y), int(draw.crop_x), int(draw.rot90)
+    # the crop's rows [cy, cy + oh) and columns [cx, cx + ow) of the rotated extent, on the flipped
+    # source: (first row, rows, first column, columns)
+    if k == 0:
+        y, h, x, w = cy, oh, cx, ow
+    elif k == 1:                                 # y = c, x = W - 1 - r
+        y, h, x, w = cx, ow, W - cy - oh, oh
+    elif k == 2:                                 # y = H - 1 - r, x = W - 1 - c
+        y, h, x, w = H - cy - oh, oh, W - cx - ow, ow
+    elif k == 3:                                 # y = H - 1 - c, x = r
+        y, h, x, w = H - cx - ow, ow, cy, oh
+    else:
+        raise ValueError(f"rot90 must be 0..3, got {k}")
+    if draw.flipud:
+        y = H - y - h
+    if draw.fliplr:
+        x = W - x - w
+    if y < 0 or x < 0 or y + h > H or x + w > W:
+        raise ValueError(f"the {oh}x{ow} crop at ({cy}, {cx}) with rot90 {k} lies outside the {H}x{W} source")
+    return y, x, h, w
+
+
 def _check_source(t, what):
     if not isinstance(t, torch.Tensor) or t.dtype not in _TORCH_FMT or t.dim() != 3 or t.shape[2] != 3:
         raise ValueError(f"{what} must be a [H, W, 3] uint8 / uint16 / float32 tensor")
@@ -216,22 +258,56 @@ def train_batch(inputs, targets, draws, output_resolution, size: int, out=None):
     return out
 
 
+ALIGN = 256           # byte alignment of every image in the device cache and of every staged window
+STREAM_SLOTS = 2      # pinned and device staging slots of the streamed tier
+
+
+def _aligned(nbytes: int) -> int:
+    return -(-int(nbytes) // ALIGN) * ALIGN
+
+
+def cache_bytes(images) -> int:
+    """Bytes of the device tier's cache of ``images`` (each starts 256-byte aligned)."""
+    return sum(_aligned(im.nbytes) for im in images)
+
+
+def slot_bytes(formats, batch_size: int, output_resolution) -> int:
+    """Bytes of one staging slot of the streamed tier: ``batch_size`` samples of the widest
+    (input dtype, target dtype) pair in ``formats``, each window of oh x ow pixels 256-byte aligned."""
+    oh, ow = (int(v) for v in output_resolution)
+    widest = max(_aligned(oh * ow * 3 * np.dtype(a).itemsize) + _aligned(oh * ow * 3 * np.dtype(b).itemsize)
+                 for a, b in formats)
+    return int(batch_size) * widest
+
+
+def device_budget(device) -> int:
+    """Free device memory on ``device`` in bytes, as the tier selection sees it."""
+    return torch.cuda.mem_get_info(device)[0]
+
+
+def choose_tier(dataset_bytes: int, staging_bytes: int, device, margin: int = MEMORY_MARGIN) -> str:
+    """``"device"`` when the dataset fits in ``device_budget(device) - margin``, else ``"stream"``
+    when the staging slots do; MemoryError, naming the byte counts, when neither fits."""
+    free = device_budget(device)
+    available = free - margin
+    if dataset_bytes <= available:
+        return "device"
+    if staging_bytes <= available:
+        return "stream"
+    raise MemoryError(
+        f"the dataset needs {dataset_bytes} bytes of device memory and streaming it from the host needs "
+        f"{staging_bytes} bytes of staging slots; {free} bytes are free and {margin} are kept for training, so "
+        f"{max(available, 0)} are available: use a smaller batch or output resolution")
+
+
 class DeviceCache:
     """Decoded images in one device buffer, each in its own storage format."""
 
-    ALIGN = 256
-
-    def __init__(self, images, device, margin: int = MEMORY_MARGIN):
+    def __init__(self, images, device):
         offsets, total = [], 0
         for im in images:
             offsets.append(total)
-            total += -(-im.nbytes // self.ALIGN) * self.ALIGN
-        free, _ = torch.cuda.mem_get_info(device)
-        if total > free - margin:
-            raise MemoryError(
-                f"the dataset needs {total} bytes of device memory; {free} bytes are free and {margin} are kept "
-                f"for training, so {max(free - margin, 0)} are available.  Streaming from the host is not "
-                "implemented: use fewer or smaller images")
+            total += _aligned(im.nbytes)
         self.nbytes = total
         self.buffer = torch.empty(total, dtype=torch.uint8, device=device)
         self.images = []
@@ -242,12 +318,180 @@ class DeviceCache:
             self.images.append(dst.view(getattr(torch, im.dtype.name)).view(im.shape))
 
 
+class _Staged(NamedTuple):
+    """A batch in device slot ``slot``: each sample's (input, target) window views and its draw with
+    the crop at the window's origin; ``uploaded`` is the event of the slot's copy."""
+    slot: int
+    inputs: list
+    targets: list
+    draws: list
+    uploaded: object
+
+
+class HostStream:
+    """The streamed tier: decoded pairs on the host, each batch's crop windows staged through
+    ``STREAM_SLOTS`` pinned and device slots by a producer thread, packed by ``nthreads`` workers.
+
+    A device slot is reused only after the batch kernel that read it has been enqueued (its
+    ``consumed`` event recorded on the consumer's stream; the copy stream waits on it), and a pinned
+    slot only after its previous upload has completed (the producer waits on the host)."""
+
+    def __init__(self, inputs, targets, sampler, output_resolution, device, nthreads=1):
+        self.inputs, self.targets, self.sampler = inputs, targets, sampler
+        self.oh, self.ow = (int(v) for v in output_resolution)
+        self.device = device
+        self.slot_bytes = slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)}, sampler.batch_size,
+                                     output_resolution)
+        with torch.cuda.device(device):
+            self.copy_stream = torch.cuda.Stream(device)
+            with torch.cuda.stream(self.copy_stream):     # the blocks belong to the stream that writes them
+                self.dev = [torch.empty(self.slot_bytes, dtype=torch.uint8, device=device)
+                            for _ in range(STREAM_SLOTS)]
+            self.pinned = [torch.empty(self.slot_bytes, dtype=torch.uint8, pin_memory=True)
+                           for _ in range(STREAM_SLOTS)]
+            self.uploaded = [torch.cuda.Event() for _ in range(STREAM_SLOTS)]
+        self.consumed = [None] * STREAM_SLOTS              # event: the last batch kernel that read the slot
+        self.busy = [False] * STREAM_SLOTS                 # the slot holds a batch not yet consumed
+        self.ready = {}                                    # step -> _Staged or the exception that built it
+        self.filling = None                                # (step, generation) being built
+        self.next = None                                   # next step to build; None: idle
+        self.generation = 0
+        self.closed = False
+        self.pack_seconds, self.packed = 0.0, 0            # host time copying windows, batches packed
+        self.cond = threading.Condition()
+        self.pool = concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads)),
+                                                          thread_name_prefix="hdrnet-stream-pack")
+        self.thread = threading.Thread(target=self._produce, name="hdrnet-stream", daemon=True)
+        self.thread.start()
+
+    # ---- producer ------------------------------------------------------------------------------
+    def _pack(self, slot: int, step: int) -> _Staged:
+        """Copy batch ``step``'s windows into pinned slot ``slot`` and upload it to device slot
+        ``slot`` on the copy stream."""
+        draws = self.sampler.draws(step)
+        layout, off = [], 0
+        for d in draws:
+            a, b = self.inputs[d.index], self.targets[d.index]
+            y0, x0, h, w = source_window(a.shape[0], a.shape[1], d, self.oh, self.ow)
+            na, nb = h * w * 3 * a.itemsize, h * w * 3 * b.itemsize
+            layout.append((d, (y0, x0, h, w), off, off + _aligned(na)))
+            off += _aligned(na) + _aligned(nb)
+        self.uploaded[slot].synchronize()                  # the pinned slot's last upload has completed
+        host = self.pinned[slot].numpy()
+
+        def copy(item):
+            d, (y0, x0, h, w), oa, ob = item
+            for src, o in ((self.inputs[d.index], oa), (self.targets[d.index], ob)):
+                dst = host[o:o + h * w * 3 * src.itemsize].view(src.dtype).reshape(h, w, 3)
+                np.copyto(dst, src[y0:y0 + h, x0:x0 + w])
+
+        t0 = time.perf_counter()
+        list(self.pool.map(copy, layout))
+        self.pack_seconds += time.perf_counter() - t0
+        self.packed += 1
+        with torch.cuda.device(self.device), torch.cuda.stream(self.copy_stream):
+            if self.consumed[slot] is not None:
+                self.copy_stream.wait_event(self.consumed[slot])
+            self.dev[slot][:off].copy_(self.pinned[slot][:off], non_blocking=True)
+            self.uploaded[slot].record(self.copy_stream)
+        dev = self.dev[slot]
+        inputs, targets, crops = [], [], []
+        for d, (_, _, h, w), oa, ob in layout:
+            a, b = self.inputs[d.index], self.targets[d.index]
+            inputs.append(dev[oa:oa + h * w * 3 * a.itemsize].view(getattr(torch, a.dtype.name)).view(h, w, 3))
+            targets.append(dev[ob:ob + h * w * 3 * b.itemsize].view(getattr(torch, b.dtype.name)).view(h, w, 3))
+            crops.append(d._replace(crop_y=0, crop_x=0))
+        return _Staged(slot, inputs, targets, crops, self.uploaded[slot])
+
+    def _produce(self):
+        while True:
+            with self.cond:
+                while not self.closed and (self.next is None or all(self.busy)):
+                    self.cond.wait()
+                if self.closed:
+                    return
+                step, gen = self.next, self.generation
+                slot = self.busy.index(False)
+                self.busy[slot] = True
+                self.filling = (step, gen)
+                self.next = step + 1
+            try:
+                item = self._pack(slot, step)
+            except BaseException as e:          # handed to the batch() that asks for this step
+                item = e
+            with self.cond:
+                self.filling = None
+                if gen != self.generation:
+                    self.busy[slot] = False     # built for a sequence that was restarted
+                else:
+                    self.ready[step] = item
+                    if isinstance(item, BaseException):
+                        self.busy[slot] = False
+                        self.next = None        # stop building ahead after a failure
+                self.cond.notify_all()
+
+    # ---- consumer ------------------------------------------------------------------------------
+    def _release(self, step):
+        item = self.ready.pop(step)
+        if isinstance(item, _Staged):
+            self.busy[item.slot] = False
+
+    def take(self, step: int) -> _Staged:
+        """Batch ``step``'s staged windows, built ahead when ``step`` follows the last request, else
+        built now (and building ahead restarts from ``step + 1``)."""
+        step = int(step)
+        with self.cond:
+            if self.closed:
+                raise RuntimeError("the data pipeline is closed")
+            expected = step in self.ready or (self.filling is not None and self.filling == (step, self.generation))
+            for s in [s for s in self.ready if s < step or not expected]:
+                self._release(s)
+            if not expected:
+                self.generation += 1
+                self.next = step
+            self.cond.notify_all()
+            with torch.profiler.record_function("data_pipeline.stream.wait"):
+                while step not in self.ready:
+                    self.cond.wait()
+            item = self.ready[step]
+            if isinstance(item, BaseException):
+                self.ready.pop(step)
+                raise item
+            if self.next is None:
+                self.next = step + 1
+            return item
+
+    def consumed_by(self, item: _Staged, stream) -> None:
+        """The batch kernel that reads ``item`` has been enqueued on ``stream``: the slot may be
+        refilled once it has run."""
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        self.dev[item.slot].record_stream(stream)
+        with self.cond:
+            self.consumed[item.slot] = ev
+            for s, it in list(self.ready.items()):
+                if it is item:
+                    self._release(s)
+            self.cond.notify_all()
+
+    def close(self) -> None:
+        with self.cond:
+            if self.closed:
+                return
+            self.closed = True
+            self.cond.notify_all()
+        self.thread.join()
+        self.pool.shutdown(wait=True)
+        self.copy_stream.synchronize()
+
+
 class ImageFilesDataPipeline:
     """The reference's ImageFilesDataPipeline on the device (keyword names of data_pipeline.py:71-82).
 
     ``batch(step)`` returns the reference's sample dict for training step ``step``: ``image_input``,
     ``image_output`` [B, oh, ow, 3] and ``lowres_input`` [B, S, S, 3], float32 on ``device``, with
-    S = ``params['net_input_size']`` (256 without params)."""
+    S = ``params['net_input_size']`` (256 without params).  ``tier`` is ``"device"`` or ``"stream"``
+    (module docstring); ``close()`` (or leaving a ``with`` block) stops the streamed tier's threads."""
 
     def __init__(self, path, batch_size=32, output_resolution=(1080, 1920), shuffle=False, fliplr=False,
                  flipud=False, rotate=False, random_crop=False, params=None, nthreads=1, seed=0, device=None,
@@ -263,13 +507,49 @@ class ImageFilesDataPipeline:
         self.sampler = Sampler([a.shape[:2] for a in inputs], batch_size, self.output_resolution, shuffle,
                                fliplr, flipud, rotate, random_crop, seed)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        cache = DeviceCache([im for pair in zip(inputs, targets) for im in pair], self.device, memory_margin)
-        self.cache = cache
-        self.inputs, self.targets = cache.images[0::2], cache.images[1::2]
-        log.info("%s: %d pairs, %.1f MB on %s", dirname, self.nsamples, cache.nbytes / 1e6, self.device)
+        images = [im for pair in zip(inputs, targets) for im in pair]
+        self.dataset_bytes = cache_bytes(images)
+        self.staging_bytes = STREAM_SLOTS * slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)},
+                                                       self.batch_size, self.output_resolution)
+        self.tier = choose_tier(self.dataset_bytes, self.staging_bytes, self.device, memory_margin)
+        self.stream = None
+        if self.tier == "device":
+            cache = DeviceCache(images, self.device)
+            self.cache = cache
+            self.inputs, self.targets = cache.images[0::2], cache.images[1::2]
+            log.info("%s: %d pairs, %.1f MB on %s", dirname, self.nsamples, cache.nbytes / 1e6, self.device)
+        else:
+            self.stream = HostStream(inputs, targets, self.sampler, self.output_resolution, self.device, nthreads)
+            log.info("%s: %d pairs, %.1f MB: more than the %.1f MB of %s's free memory less the %.1f MB kept "
+                     "for training, so they stay on the host and each batch's crops are streamed through %d "
+                     "staging slots of %.1f MB", dirname, self.nsamples, self.dataset_bytes / 1e6,
+                     device_budget(self.device) / 1e6, self.device, memory_margin / 1e6, STREAM_SLOTS,
+                     self.stream.slot_bytes / 1e6)
 
     def batch(self, step: int) -> dict:
-        draws = self.sampler.draws(step)
-        fin, fout, low = train_batch([self.inputs[d.index] for d in draws], [self.targets[d.index] for d in draws],
-                                     draws, self.output_resolution, self.net_input_size)
+        if self.stream is None:
+            draws = self.sampler.draws(step)
+            fin, fout, low = train_batch([self.inputs[d.index] for d in draws],
+                                         [self.targets[d.index] for d in draws],
+                                         draws, self.output_resolution, self.net_input_size)
+            return {"image_input": fin, "image_output": fout, "lowres_input": low}
+        item = self.stream.take(step)
+        stream = torch.cuda.current_stream(self.device)
+        stream.wait_event(item.uploaded)
+        try:
+            fin, fout, low = train_batch(item.inputs, item.targets, item.draws, self.output_resolution,
+                                         self.net_input_size)
+        finally:
+            self.stream.consumed_by(item, stream)
         return {"image_input": fin, "image_output": fout, "lowres_input": low}
+
+    def close(self) -> None:
+        """Stop and join the streamed tier's threads (nothing to do on the device tier)."""
+        if self.stream is not None:
+            self.stream.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()

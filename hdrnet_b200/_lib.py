@@ -49,6 +49,14 @@ SIGNATURES = {
     "hdrnet_guide_curves_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong]),
     "hdrnet_guide_curves_grad_f32": (_c_int, [_vp] * 3 + [ctypes.c_longlong] + [_vp] * 5
                                      + [ctypes.c_float, _vp, _vp, ctypes.c_size_t, _vp]),
+    # (input, npix, moments, ws, bytes, stream); (w1, beta, moments, feats, w1_folded, b1_folded, mean, var)
+    "hdrnet_guide_nn_stats_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong]),
+    "hdrnet_guide_nn_stats_f32": (_c_int, [_vp, ctypes.c_longlong, _vp, _vp, ctypes.c_size_t, _vp]),
+    "hdrnet_guide_nn_batch_fold": (_c_int, [_vp] * 3 + [_c_int] + [_vp] * 4),
+    # (input, dguide, dinput, npix, w1, beta, w2, b2, feats, moments, dparams, ws, bytes, stream)
+    "hdrnet_guide_nn_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong, _c_int]),
+    "hdrnet_guide_nn_grad_f32": (_c_int, [_vp] * 3 + [ctypes.c_longlong] + [_vp] * 3
+                                 + [ctypes.c_float, _c_int, _vp, _vp, _vp, ctypes.c_size_t, _vp]),
     "hdrnet_slice_apply_curves_f32": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 5 + [ctypes.c_float, _vp]),
     "hdrnet_slice_apply_nn_f32": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 3 + [ctypes.c_float, _c_int, _vp]),
     "hdrnet_slice_apply_curves_f32_ws": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 5

@@ -5,7 +5,7 @@ arguments, flags and defaults (train.py:188-244):
     python -m hdrnet_b200.bin.train <checkpoint_dir> <data_dir> [--eval_data_dir DIR]
         [--learning_rate 1e-4] [--batch_size 16] [--[no]fliplr|flipud|rotate|random_crop]
         [--model_name HDRNetCurves] [--net_input_size 256] [--output_resolution 512 512] ...
-        [--max_steps N] [--seed S] [--[no]train_guide]
+        [--max_steps N] [--seed S] [--[no]train_guide] [--[no]guide_batch_stats]
 
 ``data_dir`` holds ``filelist.txt`` and the ``input/`` and ``output/`` folders (or is that
 ``filelist.txt``); hdrnet_b200/data_pipeline.py decodes the pairs once and builds each batch in one
@@ -33,14 +33,28 @@ same Adam at the same learning rate, as the reference's single ``opt.minimize`` 
 (train.py:92-94, :115); their Adam slots then go into each checkpoint.  Without the flag (the
 default) the guide variables are held fixed at their initial (or restored) values.  A resume whose
 checkpoint was written with the other setting of the flag is refused before any data is read.
-Training-mode batch norm and the pyramid's resize VJP are not implemented, so ``--batch_norm``,
-``HDRNetGaussianPyrNN`` and ``--train_guide`` with ``HDRNetPointwiseNNGuide`` (whose guide has batch
-norm) are refused before any data is read, with the models' own ``NotImplementedError``.
+
+``HDRNetPointwiseNNGuide``'s guide has batch norm after conv1, which the reference trains in training
+mode.  ``--guide_batch_stats`` runs each step's forward that way (``inference(..., is_training=True)``):
+conv1 is normalised with the batch's statistics, and ``conv1/BatchNorm/moving_mean`` and
+``moving_variance`` move toward them once per step (decay 0.999), as the reference's ``UPDATE_OPS``
+do (train.py:110-115).  The evaluation, and ``bin/run.py`` on the checkpoints, use the moving
+averages, as the reference's eval graph does.  ``--train_guide --guide_batch_stats`` trains the whole
+model as the reference's ``*_nn.sh`` scripts do.  The moving averages are not trainable: they get no
+Adam slots, but go into every checkpoint and are restored on resume.  The flag is not a model
+parameter and is not written to ``params.json``; a checkpoint does not record it, so a resume with the
+other setting is not refused: it only changes the guide's forward from then on.  ``--train_guide``
+with this model needs the flag; ``--guide_batch_stats`` with ``HDRNetCurves`` (no batch norm) is
+refused with ``ValueError``.  Training-mode batch norm in the coefficient network and the pyramid's
+resize VJP are not implemented, so ``--batch_norm``, ``HDRNetGaussianPyrNN`` and ``--train_guide``
+with ``HDRNetPointwiseNNGuide`` without ``--guide_batch_stats`` are refused before any data is read,
+with the models' own ``NotImplementedError``.
 
 Deliberate differences from the reference:
 
-* ``--max_steps`` (the reference runs until interrupted), ``--seed`` and ``--train_guide`` are added
-  (the reference always trains the guide; here it is opt-in);
+* ``--max_steps`` (the reference runs until interrupted), ``--seed``, ``--train_guide`` and
+  ``--guide_batch_stats`` are added (the reference always trains the guide, in training mode; here
+  both are opt-in);
   ``--data_pipeline`` takes only ``ImageFilesDataPipeline`` (the tfrecord pipelines need TF);
   ``--profiling`` is accepted and ignored.
 * The evaluation reads ``--eval_data_dir``.  The reference builds the eval pipeline but then
@@ -98,6 +112,10 @@ def build_parser() -> argparse.ArgumentParser:
     train_grp.add_argument("--train_guide", dest="train_guide", action="store_true",
                            help="train the curves guide's variables too, as the reference does (HDRNetCurves only).")
     train_grp.add_argument("--notrain_guide", dest="train_guide", action="store_false")
+    train_grp.add_argument("--guide_batch_stats", dest="guide_batch_stats", action="store_true",
+                           help="run the pointwise-NN guide's batch norm in training mode (batch statistics, "
+                                "moving averages updated), as the reference does (HDRNetPointwiseNNGuide only).")
+    train_grp.add_argument("--noguide_batch_stats", dest="guide_batch_stats", action="store_false")
 
     debug_grp = parser.add_argument_group("debug and profiling")
     debug_grp.add_argument("--profiling", dest="profiling", action="store_true", help="accepted for compatibility; ignored.")
@@ -131,7 +149,7 @@ def build_parser() -> argparse.ArgumentParser:
     model_grp.add_argument("--spatial_bin", default=16, type=int, help="Size of the spatial BGU bins (pixels).")
 
     parser.set_defaults(profiling=False, flipud=False, fliplr=False, rotate=False, random_crop=True, batch_norm=False,
-                        train_guide=False)
+                        train_guide=False, guide_batch_stats=False)
     parser.model_group = model_grp
     return parser
 
@@ -141,11 +159,12 @@ def model_params(parser, args) -> dict:
     return {a.dest: getattr(args, a.dest, None) for a in parser.model_group._group_actions}
 
 
-def refuse_untrainable(params, train_guide=False) -> None:
+def refuse_untrainable(params, train_guide=False, guide_batch_stats=False) -> None:
     """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model,
-    training-mode batch norm and (with ``train_guide``) the pointwise-NN guide.  Asks the models
-    themselves, on the CPU, with a stand-in variable that requires grad (they refuse before any
-    device work)."""
+    training-mode batch norm in the coefficient network and (with ``train_guide``) the pointwise-NN
+    guide without ``guide_batch_stats``.  Asks the models themselves, on the CPU, with a stand-in
+    variable that requires grad (they refuse before any device work).  ValueError for
+    ``guide_batch_stats`` on ``HDRNetCurves``, whose guide has no batch norm."""
     S = int(params["net_input_size"])
     if params["model_name"] == "HDRNetGaussianPyrNN":
         probe = {COEFFS + "splat/conv1/weights": torch.zeros(1, requires_grad=True)}
@@ -155,10 +174,16 @@ def refuse_untrainable(params, train_guide=False) -> None:
         probe = {f"{scope}/BatchNorm/beta": torch.zeros(1, requires_grad=True)
                  for scope, use_bn, _ in models._coefficient_specs(params) if use_bn}
         getattr(models, params["model_name"])._coefficients(torch.zeros(1, S, S, 3), dict(params, weights=probe))
-    if train_guide and params["model_name"] == "HDRNetPointwiseNNGuide":
+    if guide_batch_stats and params["model_name"] == "HDRNetCurves":
+        raise ValueError("--guide_batch_stats runs the pointwise-NN guide's batch norm in training mode; "
+                         "HDRNetCurves' guide has no batch norm")
+    if train_guide and not guide_batch_stats and params["model_name"] == "HDRNetPointwiseNNGuide":
         probe = {GUIDE + "conv2/weights": torch.zeros(1, requires_grad=True)}
-        models.HDRNetPointwiseNNGuide.inference(torch.zeros(1, S, S, 3), torch.zeros(1, 1, 1, 3),
-                                                dict(params, weights=probe, guide_grad=True))
+        try:
+            models.HDRNetPointwiseNNGuide.inference(torch.zeros(1, S, S, 3), torch.zeros(1, 1, 1, 3),
+                                                    dict(params, weights=probe, guide_grad=True))
+        except NotImplementedError as e:
+            raise NotImplementedError(f"{e}; --guide_batch_stats runs it in training mode and trains it") from None
 
 
 def refuse_resume_mismatch(saved: dict, train_guide: bool) -> None:
@@ -171,6 +196,14 @@ def refuse_resume_mismatch(saved: dict, train_guide: bool) -> None:
     if has_slots and not train_guide:
         raise ValueError("the checkpoint to resume was trained with --train_guide (it holds Adam slots for "
                          "inference/guide/*): resume it with --train_guide")
+
+
+def trained_names(variables, train_guide=False):
+    """The variables Adam trains: the coefficient network's, and with ``train_guide`` the guide's;
+    never a batch norm's ``moving_mean`` / ``moving_variance``, which the training-mode forward
+    updates (TF does not train them)."""
+    prefixes = (COEFFS, GUIDE) if train_guide else (COEFFS,)
+    return sorted(k for k in variables if k.startswith(prefixes) and "/BatchNorm/moving_" not in k)
 
 
 def slot_names(name):
@@ -219,8 +252,7 @@ class Trainer:
         self.device = torch.device("cuda", torch.cuda.current_device())
         init = models.init_weights(params, seed=args.seed, model_name=params["model_name"])
         self.weights = {k: torch.from_numpy(v).to(self.device) for k, v in init.items()}
-        trained = (COEFFS, GUIDE) if args.train_guide else (COEFFS,)
-        self.names = sorted(k for k in self.weights if k.startswith(trained))
+        self.names = trained_names(self.weights, args.train_guide)
         for k in self.names:
             self.weights[k].requires_grad_(True)
         self.opt = torch.optim.Adam([self.weights[k] for k in self.names], lr=args.learning_rate,
@@ -247,6 +279,10 @@ class Trainer:
         self.p = dict(params, weights=self.weights)
         if args.train_guide:
             self.p["guide_grad"] = True
+        self.is_training = bool(getattr(args, "guide_batch_stats", False))
+        if self.is_training:
+            log.info("%s: the guide's batch norm runs in training mode (batch statistics; moving averages "
+                     "updated each step)", params["model_name"])
 
     # ---- checkpoints ---------------------------------------------------------------------------
     def _resume(self):
@@ -287,7 +323,8 @@ class Trainer:
         """One gradient step on batch ``self.step``; returns (loss, psnr) as device scalars."""
         batch = self.train_data.batch(self.step)
         self.opt.zero_grad(set_to_none=True)
-        pred = self.mdl.inference(batch["lowres_input"], batch["image_input"], self.p)
+        pred = self.mdl.inference(batch["lowres_input"], batch["image_input"], self.p,
+                                  is_training=self.is_training)
         loss = metrics.l2_loss(batch["image_output"], pred)
         with torch.no_grad():
             psnr = metrics.psnr(batch["image_output"], pred)
@@ -358,7 +395,7 @@ def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
     params = model_params(parser, args)
-    refuse_untrainable(params, args.train_guide)     # before any data is read
+    refuse_untrainable(params, args.train_guide, args.guide_batch_stats)     # before any data is read
     prefix = checkpoint.latest_checkpoint(args.checkpoint_dir)
     if prefix is not None:
         refuse_resume_mismatch(checkpoint.read_tf_checkpoint(prefix), args.train_guide)

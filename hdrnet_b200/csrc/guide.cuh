@@ -70,6 +70,24 @@ __device__ __forceinline__ float curves_guide(const CurvesGuideParams& p, float 
   return fminf(fmaxf(curves_guide_preclip(p, r, g, b, t), 0.0f), 1.0f);
 }
 
+// The pointwise-NN guide in pieces, so that its VJP (guide_nn_grad.cu) recomputes the forward's
+// own floats: nn_guide_preact2 is the pre-activation of features f and f + 1 (its relu masks),
+// nn_guide_sigmoid the output from the two lanes of sum_f relu(h_f) w2_f.
+__device__ __forceinline__ unsigned long long nn_guide_preact2(const NNGuideParams& p, unsigned long long r2,
+                                                               unsigned long long g2, unsigned long long b2v,
+                                                               int f) {
+  unsigned long long h2 = fma2(r2, pack2(p.w1[0][f], p.w1[0][f + 1]), pack2(p.b1[f], p.b1[f + 1]));
+  h2 = fma2(g2, pack2(p.w1[1][f], p.w1[1][f + 1]), h2);
+  return fma2(b2v, pack2(p.w1[2][f], p.w1[2][f + 1]), h2);
+}
+
+__device__ __forceinline__ float nn_guide_sigmoid(const NNGuideParams& p, unsigned long long y2) {
+  float y0, y1;
+  unpack2(y2, y0, y1);
+  const float y = (y0 + y1) + p.b2;
+  return __fdividef(1.0f, 1.0f + __expf(-y));
+}
+
 // kFeats is a compile-time bound (16 or 32): the loop unrolls fully and every weight is a
 // constant-bank operand with a static offset (a runtime feature count costs an indexed LDC per
 // weight).  Weights beyond p.feats are zero (pack_nn_params), so the extra features add 0.
@@ -80,17 +98,11 @@ __device__ __forceinline__ float nn_guide(const NNGuideParams& p, float r, float
   unsigned long long y2 = 0ull;
 #pragma unroll
   for (int f = 0; f < kFeats; f += 2) {
-    unsigned long long h2 = fma2(r2, pack2(p.w1[0][f], p.w1[0][f + 1]), pack2(p.b1[f], p.b1[f + 1]));
-    h2 = fma2(g2, pack2(p.w1[1][f], p.w1[1][f + 1]), h2);
-    h2 = fma2(b2v, pack2(p.w1[2][f], p.w1[2][f + 1]), h2);
     float h0, h1;
-    unpack2(h2, h0, h1);
+    unpack2(nn_guide_preact2(p, r2, g2, b2v, f), h0, h1);
     y2 = fma2(pack2(fmaxf(h0, 0.0f), fmaxf(h1, 0.0f)), pack2(p.w2[f], p.w2[f + 1]), y2);
   }
-  float y0, y1;
-  unpack2(y2, y0, y1);
-  const float y = (y0 + y1) + p.b2;
-  return __fdividef(1.0f, 1.0f + __expf(-y));
+  return nn_guide_sigmoid(p, y2);
 }
 
 }  // namespace hdrnet_b200

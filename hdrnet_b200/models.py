@@ -26,9 +26,14 @@ hdrnet/bin/train.py:224-236) that is the coefficient network's training graph.  
 ``params['guide_grad']`` truthy, ``HDRNetCurves``'s guide variables (``ccm``, ``ccm_bias``,
 ``shifts``, ``slopes``, ``channel_mixing/*``) and ``fullres_input`` are differentiated too, through
 ``_CurvesGuideFn`` and the VJP of ``csrc/guide_grad.cu``; without the key, asking for their gradient
-raises ``NotImplementedError`` as before.  The pointwise-NN guide (its conv1 has batch norm, which
-training runs in training mode), batch-norm layers and the pyramid model's resize are not
-differentiated: asking for their gradient raises ``NotImplementedError``.
+raises ``NotImplementedError`` as before.  The pointwise-NN guide's conv1 has batch norm, which
+training runs in training mode: ``HDRNetPointwiseNNGuide.inference(..., is_training=True)`` is the
+reference's training graph, with conv1 normalised by the batch's statistics
+(``csrc/guide_nn_grad.cu``), its moving averages updated in place on every call, and, with
+``params['guide_grad']``, gradients for the guide's variables and ``fullres_input`` through
+``_NNGuideFn``.  In the inference form (``is_training=False``) that guide is not differentiated.
+Batch-norm layers of the coefficient network and the pyramid model's resize are not differentiated:
+asking for their gradient raises ``NotImplementedError``.
 
 Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
   coefficients  4 splat convs, 2 global convs + 3 FCs, 2 local convs (conv2d / fc kernels),
@@ -52,6 +57,7 @@ __all__ = ["HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN", "set
            "init_weights", "DEFAULT_PARAMS"]
 
 BN_EPS = 1e-3   # tf.contrib.layers.batch_norm default epsilon (hdrnet/layers.py:47-54)
+BN_DECAY = 0.999  # ... and its moving-average decay
 
 DEFAULT_PARAMS = dict(  # hdrnet/bin/train.py:224-236
     model_name="HDRNetCurves", net_input_size=256, output_resolution=[512, 512],
@@ -643,6 +649,125 @@ def _curves_guide_grad(wts, params, x) -> bool:
                                  any(_requires_grad(wts.get("inference/guide/" + n)) for n in _CURVES_VARS))
 
 
+_NN_GUIDE_VARS = ("conv1/weights", "conv1/BatchNorm/beta", "conv2/weights", "conv2/biases")
+_NN_MOVING = ("conv1/BatchNorm/moving_mean", "conv1/BatchNorm/moving_variance")
+
+
+class _BatchStats(collections.namedtuple("_BatchStats", "npix moments w1f b1f mean var host")):
+    """conv1's batch statistics of one training-mode call: the input's moments (float64 [9]), the
+    folded float32 weights the guide kernel runs with, the features' batch mean and biased variance
+    (float64), and the host copies (_host_f32) of the four variables they were folded from."""
+
+
+def _nn_batch_stats(x, host) -> _BatchStats:
+    """hdrnet_guide_nn_stats_f32 over x [B,H,W,3] (contiguous), one device-to-host copy of the 9
+    moments, then hdrnet_guide_nn_batch_fold in float64 on the host."""
+    lib = _lib.load()
+    npix = x.numel() // 3
+    w1, beta = host[0], host[1]
+    feats = beta.size
+    moments = torch.empty(9, dtype=torch.float64, device=x.device)
+    ws = _grad_workspace(x.device, lib.hdrnet_guide_nn_stats_workspace_bytes(npix))
+    rc = lib.hdrnet_guide_nn_stats_f32(x.data_ptr(), npix, moments.data_ptr(), ws.data_ptr(), ws.numel() * 4,
+                                       _stream(x.device))
+    _lib.check(rc, "guide_nn batch statistics")
+    mom = np.ascontiguousarray(moments.cpu().numpy())
+    w1f, b1f = np.empty(3 * feats, np.float32), np.empty(feats, np.float32)
+    mean, var = np.empty(feats, np.float64), np.empty(feats, np.float64)
+    rc = lib.hdrnet_guide_nn_batch_fold(_hp(w1), _hp(beta), _hp(mom), feats, _hp(w1f), _hp(b1f), _hp(mean), _hp(var))
+    _lib.check(rc, "guide_nn batch-norm fold")
+    return _BatchStats(npix, mom, w1f, b1f, mean, var, host)
+
+
+def _update_moving_averages(moving, stats: _BatchStats) -> None:
+    """moving_mean and moving_variance toward the batch's statistics, in place, as TF's
+    assign_moving_average without zero-debias: v -= (1 - decay) (v - batch).  The variance fed to it
+    is Bessel-corrected, var N / (N - 1) (1 for N = 1), as TF's fused batch norm does (DESIGN.md §5)."""
+    n = stats.npix
+    unbiased = stats.var * (n / (n - 1.0) if n > 1 else 1.0)
+    with torch.no_grad():
+        for v, batch in zip(moving, (stats.mean, unbiased)):
+            b = torch.from_numpy(batch.astype(np.float32)).to(v.device).reshape(v.shape)
+            v.sub_((v - b) * (1.0 - BN_DECAY))
+
+
+def _moving_averages(wts):
+    """The guide's moving averages, which training mode updates in place: float32 tensors that do not
+    require grad (TF does not train them)."""
+    out = []
+    for n in _NN_MOVING:
+        key = "inference/guide/" + n
+        v = wts.get(key) if isinstance(wts, dict) else None
+        if not isinstance(v, torch.Tensor) or v.dtype != torch.float32:
+            raise TypeError(f"{key} must be a float32 torch.Tensor: is_training=True updates it in place "
+                            f"(got {type(v).__name__ if not isinstance(v, torch.Tensor) else v.dtype})")
+        if v.requires_grad:
+            raise ValueError(f"{key} requires grad: moving averages are not trainable; is_training=True "
+                             "updates them in place")
+        out.append(v)
+    return out
+
+
+def _launch_nn_guide(x, w1, b1, w2, b2, feats) -> torch.Tensor:
+    """hdrnet_guide_nn_f32 with host weights (conv1's batch norm already folded) -> [B, H, W]."""
+    B, H, W, _ = x.shape
+    guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
+    rc = _lib.load().hdrnet_guide_nn_f32(x.data_ptr(), guide.data_ptr(), B * H * W, _hp(w1), _hp(b1), _hp(w2),
+                                         float(b2), int(feats), _stream(x.device))
+    _lib.check(rc, "guide_nn")
+    return guide
+
+
+class _NNGuideFn(torch.autograd.Function):
+    """The pointwise-NN guide in training mode (hdrnet/models.py:203-210, batch norm with the batch's
+    statistics) over x and its four variables (_NN_GUIDE_VARS order); `stats` is _nn_batch_stats of
+    x.  Forward: the existing guide kernel on the folded weights.  Backward:
+    hdrnet_guide_nn_grad_f32, whose gradients include the paths through the batch mean and variance."""
+
+    @staticmethod
+    def forward(ctx, x, w1, beta, w2, b2, stats):
+        x = x.contiguous()
+        host = stats.host
+        guide = _launch_nn_guide(x, stats.w1f, stats.b1f, host[2], host[3][0], host[1].size)
+        ctx.save_for_backward(x)
+        ctx.stats = stats
+        ctx.vars = [(v.shape, v.device) if isinstance(v, torch.Tensor) else None for v in (w1, beta, w2, b2)]
+        return guide
+
+    @staticmethod
+    def backward(ctx, dguide):
+        (x,) = ctx.saved_tensors
+        dguide = dguide.contiguous()
+        need_x = ctx.needs_input_grad[0]
+        need_p = any(ctx.needs_input_grad[1:5])
+        st = ctx.stats
+        w1, beta, w2, b2 = st.host
+        F = beta.size
+        npix = st.npix
+        dx = torch.empty_like(x) if need_x else None
+        dp = torch.empty(5 * F + 1, dtype=torch.float32, device=x.device) if need_p else None
+        lib = _lib.load()
+        ws = _grad_workspace(x.device, lib.hdrnet_guide_nn_grad_workspace_bytes(npix, F))
+        with torch.cuda.device(x.device):
+            rc = lib.hdrnet_guide_nn_grad_f32(
+                x.data_ptr(), dguide.data_ptr(), _ptr(dx), npix, _hp(w1), _hp(beta), _hp(w2), float(b2[0]), F,
+                _hp(st.moments), _ptr(dp), ws.data_ptr(), ws.numel() * 4, _stream(x.device))
+        _lib.check(rc, "guide_nn VJP")
+        grads = []
+        slices = ((0, 3 * F), (3 * F, 4 * F), (4 * F, 5 * F), (5 * F, 5 * F + 1))
+        for need, var, (a, b) in zip(ctx.needs_input_grad[1:5], ctx.vars, slices):
+            grads.append(dp[a:b].reshape(var[0]).to(var[1], copy=True) if need and var is not None else None)
+        return (dx, *grads, None)
+
+
+def _nn_guide_grad(wts, params, x) -> bool:
+    """Whether the training-mode pointwise-NN guide goes through autograd: grad enabled,
+    params['guide_grad'] truthy, and a guide variable or the input requiring grad."""
+    if not (torch.is_grad_enabled() and isinstance(params, dict) and params.get("guide_grad")):
+        return False
+    return _requires_grad(x) or any(_requires_grad(wts.get("inference/guide/" + n)) for n in _NN_GUIDE_VARS)
+
+
 def _requires_grad(t) -> bool:
     return isinstance(t, torch.Tensor) and t.requires_grad
 
@@ -651,10 +776,12 @@ def _trainable_keys(wts, prefix: str):
     return sorted(k for k, v in wts.items() if k.startswith(prefix) and _requires_grad(v))
 
 
-def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None, nn_guide=False) -> None:
+def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None, nn_guide=False,
+                      is_training=False) -> None:
     """NotImplementedError for every gradient this package does not compute (checked before any
     device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN).  The curves
-    guide's variables and fullres_input are differentiated only with params['guide_grad']."""
+    guide's variables and fullres_input are differentiated only with params['guide_grad'], the
+    pointwise-NN guide's only with params['guide_grad'] and `is_training` (training-mode batch norm)."""
     if not torch.is_grad_enabled() or wts is None:
         return
     if what is not None:
@@ -666,12 +793,13 @@ def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=N
         return
     guide = _trainable_keys(wts, "inference/guide")
     guide_grad = bool(params.get("guide_grad")) if isinstance(params, dict) else False
-    if guide_grad and nn_guide and (guide or _requires_grad(fullres_input)):
+    if guide_grad and nn_guide and not is_training and (guide or _requires_grad(fullres_input)):
         wanted = guide[0] if guide else "fullres_input"
         raise NotImplementedError(
             f"gradients for the pointwise-NN guide variables and its fullres_input are not implemented ({wanted} "
             "requires grad): its conv1 has batch norm, which training runs in training mode with batch "
-            "statistics, a different forward")
+            "statistics, a different forward; inference(..., is_training=True) runs that forward and "
+            "differentiates it")
     hint = "; params['guide_grad'] computes them for HDRNetCurves"
     if guide and not guide_grad:
         raise NotImplementedError(f"gradients for the guide variables are not implemented ({guide[0]} requires "
@@ -919,7 +1047,55 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
     _nn_guide = True
 
     @classmethod
+    def inference(cls, lowres_input, fullres_input, params, is_training=False):
+        """models.py:43-59.  With ``is_training=True`` the reference's training graph
+        (hdrnet/bin/train.py:89-115): the guide's conv1 batch norm normalises with the batch's
+        statistics and its ``moving_mean`` / ``moving_variance`` (float32 tensors in the weights dict)
+        move toward them in place, once per call (decay 0.999).  The coefficient network is the
+        inference graph, which is its training graph without batch norm; ``params['batch_norm']``
+        raises ``NotImplementedError``.  The output comes from hdrnet_ops.bilateral_slice_apply, and
+        with ``params['guide_grad']`` the guide's variables (``conv1/weights``,
+        ``conv1/BatchNorm/beta``, ``conv2/*``) and ``fullres_input`` are differentiated through
+        _NNGuideFn; without it they are held fixed, while batch norm still uses the batch's
+        statistics."""
+        if not is_training:
+            return super().inference(lowres_input, fullres_input, params)
+        wts = _resolve_weights(params)
+        if params.get("batch_norm"):
+            raise NotImplementedError(
+                "training-mode batch norm in the coefficient network (params['batch_norm']) is not "
+                "implemented: only the guide's conv1 batch norm runs in training mode")
+        _moving_averages(wts)
+        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True)
+        fullres_input = _check_input(fullres_input, "fullres_input")
+        coeffs = cls._coefficients(lowres_input, params)
+        with torch.cuda.device(fullres_input.device):
+            guide = cls._guide(fullres_input, params, is_training=True)
+        B, gh, gw, gd = coeffs.shape[:4]
+        return bilateral_slice_apply(coeffs.reshape(B, gh, gw, gd, -1), guide, fullres_input, True)
+
+    @classmethod
     def _guide(cls, input_tensor, params, is_training=False):
+        """models.py:199-210 -> [B, H, W].  Inference form: conv1's batch norm folded from the moving
+        averages.  ``is_training=True``: normalised with the batch's statistics (_nn_batch_stats), the
+        moving averages updated in place, and differentiable (_NNGuideFn) when _nn_guide_grad says
+        so."""
+        if is_training:
+            wts = _resolve_weights(params)
+            moving = _moving_averages(wts)
+            _refuse_untrained(wts, params, fullres_input=input_tensor, nn_guide=True, is_training=True)
+            x = _check_input(input_tensor, "fullres_input")
+            if x.numel() == 0:
+                raise ValueError("fullres_input is empty: batch statistics need at least one pixel")
+            variables = [wts["inference/guide/" + n] for n in _NN_GUIDE_VARS]
+            host = [_host_f32(v) for v in variables]
+            with torch.cuda.device(x.device):
+                x = x.contiguous()
+                stats = _nn_batch_stats(x, host)
+                _update_moving_averages(moving, stats)
+                if _nn_guide_grad(wts, params, x):
+                    return _NNGuideFn.apply(x, *variables, stats)
+                return _launch_nn_guide(x, stats.w1f, stats.b1f, host[2], host[3][0], host[1].size)
         x = _check_input(input_tensor, "fullres_input")
         prep = _prepare(_resolve_weights(params), params, x.device, True)
         B, H, W, _ = x.shape

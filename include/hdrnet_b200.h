@@ -234,6 +234,52 @@ HDRNET_API int hdrnet_guide_curves_grad_f32(const float* input, const float* dgu
                                             size_t workspace_bytes, void* stream);
 
 /*
+ * Pointwise-NN guide in training mode (HDRNetPointwiseNNGuide._guide with is_training=True,
+ * hdrnet/models.py:203-210): conv1's batch norm normalises with the batch's statistics.  conv1 is
+ * 1x1 and linear from 3 channels, so the mean and variance of every feature follow from the mean m
+ * and the biased covariance C of the input's three channels:
+ *   mu_f = m . w1[:, f],  var_f = w1[:, f]' C w1[:, f],  s_f = 1 / sqrt(var_f + 1e-3)
+ * and the layer is hdrnet_guide_nn_f32 with w1'[c][f] = w1[c][f] s_f, b1'[f] = beta[f] - mu_f s_f.
+ *
+ * hdrnet_guide_nn_stats_f32: moments [9], a DEVICE array of doubles, receives m (3) and C
+ * (c00, c01, c02, c11, c12, c22) over npix pixels of input [npix, 3].  Per-CTA partials of fixed
+ * pixel chunks (the chunking depends on npix alone), each centred on its chunk, go to a caller-lent
+ * workspace of hdrnet_guide_nn_stats_workspace_bytes(npix) bytes (smaller: HDRNET_E_BAD_SHAPE) and
+ * are merged in float64 in a fixed order: no atomics, bitwise reproducible.  npix == 0 writes zeros.
+ *
+ * hdrnet_guide_nn_batch_fold: HOST arithmetic in float64, no device work.  From w1 [3][feats]
+ * (conv1/weights), beta [feats] (BatchNorm/beta) and HOST moments [9] it writes the folded
+ * w1_folded [3][feats] and b1_folded [feats] (float32, for hdrnet_guide_nn_f32) and, when not NULL,
+ * batch_mean [feats] and batch_var [feats] (the biased variance that normalises).
+ *
+ * hdrnet_guide_nn_grad_f32: the VJP of that guide, batch statistics included (the gradient flows
+ * through mu and var).  dguide [npix] is the gradient of the guide; relu masks are TF's
+ * (ReluGrad: y > 0), decided on the floats hdrnet_guide_nn_f32 computes with the folded weights.
+ *   dinput [npix, 3]     gradient of the input; NULL: not computed.
+ *   dparams [5 feats + 1] DEVICE array, the gradients of conv1/weights [3][feats], BatchNorm/beta
+ *                        [feats], conv2/weights [feats] and conv2/biases [1], in that order; NULL:
+ *                        not computed.
+ * w1, beta, w2 and moments are HOST pointers (the moments the forward used).  Gradients are
+ * written, not accumulated.  Per-CTA partial sums of fixed pixel chunks go to a caller-lent
+ * workspace of hdrnet_guide_nn_grad_workspace_bytes(npix, feats) bytes (needed when either output
+ * is wanted: dinput needs the sums too; smaller: HDRNET_E_BAD_SHAPE), added in a fixed order: no
+ * atomics, bitwise reproducible.  The workspace is scratch, undefined after the call.  npix == 0
+ * writes zero parameter gradients.  feats <= 32.
+ */
+HDRNET_API size_t hdrnet_guide_nn_stats_workspace_bytes(long long npix);
+HDRNET_API int hdrnet_guide_nn_stats_f32(const float* input, long long npix, double* moments,
+                                         void* workspace, size_t workspace_bytes, void* stream);
+HDRNET_API int hdrnet_guide_nn_batch_fold(const float* w1, const float* beta, const double* moments,
+                                          int feats, float* w1_folded, float* b1_folded,
+                                          double* batch_mean, double* batch_var);
+HDRNET_API size_t hdrnet_guide_nn_grad_workspace_bytes(long long npix, int feats);
+HDRNET_API int hdrnet_guide_nn_grad_f32(const float* input, const float* dguide, float* dinput,
+                                        long long npix, const float* w1, const float* beta,
+                                        const float* w2, float b2, int feats,
+                                        const double* moments, float* dparams, void* workspace,
+                                        size_t workspace_bytes, void* stream);
+
+/*
  * Model-path forms of slice-apply: the guide is computed per pixel INSIDE the kernel from the
  * full-res RGB (the guide map never touches HBM: 24 B/px instead of 28 B/px + a guide pass).
  * Replaces HDRNetCurves.inference / HDRNetPointwiseNNGuide.inference's `_guide` + `_output`

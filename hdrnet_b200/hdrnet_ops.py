@@ -101,6 +101,21 @@ def _texture_form_runs(device_index: int, B: int, rows: int, W: int, gh: int, gw
     return v.value in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
 
 
+def _slice_apply_workspace(dev: torch.device, B: int, rows: int, W: int, gh: int, gw: int, gd: int,
+                           n_in: int = 3, n_out: int = 3, has_offset: bool = True,
+                           variant: int = _lib.VARIANT_AUTO) -> torch.Tensor | None:
+    """The slab workspace to lend one slice-apply call on B x rows x W pixels, or None.  Only the
+    3 -> 3 op with offset and W % 4 == 0 takes one: always for a forced texture-assisted variant, for
+    AUTO where _texture_form_runs says AUTO then runs the texture-assisted kernel.  The caller keeps
+    the tensor referenced until the launch has been enqueued."""
+    tex = int(variant) in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
+    if not (n_in == 3 and n_out == 3 and has_offset and W % 4 == 0):
+        return None
+    if not (tex or (int(variant) == _lib.VARIANT_AUTO and _texture_form_runs(dev.index, B, rows, W, gh, gw, gd))):
+        return None
+    return _workspace(dev, _lib.load().hdrnet_slice_apply_workspace_bytes(B, rows, gw, gd))
+
+
 def _check_slice_args(grid, guide, grid_msg):
     if grid.dim() != 5:
         raise ValueError(grid_msg)
@@ -165,6 +180,52 @@ def _wants_grad(*ts) -> bool:
     return torch.is_grad_enabled() and any(t.requires_grad for t in ts)
 
 
+def _slice_apply_args(grid, guide, input, has_offset: bool, band=None):  # noqa: A002
+    """The reference op's argument checks (hdrnet/ops/bilateral_slice_apply_op.cc:147-193), with a
+    row band's (y_off, height) checked before the channels -> contiguous float32 grid, guide and
+    input, and n_out."""
+    grid = _f32c(grid, "grid")
+    guide = _f32c(guide, "guide")
+    input = _f32c(input, "input")  # noqa: A001
+    if grid.dim() != 5:
+        raise ValueError("Input grid should be 5D (batch_size, height, width, depth, "
+                         "output_channels * input_channels)")
+    if guide.dim() != 3:
+        raise ValueError("Guide image should be 3D (batch_size, height, width)")
+    if input.dim() != 4:
+        raise ValueError("Input image should be 4D (batch_size, height, width, input_channels)")
+    if tuple(input.shape[:3]) != tuple(guide.shape):
+        raise ValueError("Input and guide size should match.")
+    if guide.shape[0] != grid.shape[0]:
+        raise ValueError("Batch sizes should match.")
+    if band is not None and (band[0] < 0 or band[0] + input.shape[1] > band[1]):
+        raise ValueError(f"row band [{band[0]}, {band[0] + input.shape[1]}) does not fit an image of {band[1]} rows")
+    J = input.shape[-1] + (1 if has_offset else 0)
+    if grid.shape[-1] % J != 0:
+        if has_offset:
+            raise ValueError("Slicing with affine offset, grid should have "
+                             "output_channels * (input_channels + 1) channels.")
+        raise ValueError("Slicing without affine offset, grid should have "
+                         "output_channels * input_channels channels.")
+    return grid, guide, input, grid.shape[-1] // J
+
+
+def _launch_slice_apply(grid, guide, input, out, height: int, y_off: int, n_out: int,  # noqa: A002
+                        has_offset: bool, variant: int, what: str) -> torch.Tensor:
+    """Rows y_off .. y_off + rows - 1 of images `height` rows tall (input [B, rows, W, n_in]) on the
+    current stream, lent the workspace _slice_apply_workspace gives the call."""
+    B, gh, gw, gd, _ = grid.shape
+    _, rows, W, n_in = input.shape
+    with torch.cuda.device(grid.device):
+        ws = _slice_apply_workspace(grid.device, B, rows, W, gh, gw, gd, n_in, n_out, has_offset, variant)
+        rc = _lib.load().hdrnet_slice_apply_rows_f32_ws(
+            grid.data_ptr(), guide.data_ptr(), input.data_ptr(), out.data_ptr(), B, height, W, rows, y_off,
+            gh, gw, gd, n_in, n_out, int(has_offset), int(variant), 0 if ws is None else ws.data_ptr(),
+            0 if ws is None else ws.numel() * 4, torch.cuda.current_stream(grid.device).cuda_stream)
+    _lib.check(rc, what)
+    return out
+
+
 def bilateral_slice(grid: torch.Tensor, guide: torch.Tensor, name=None, *,
                     variant: int = _lib.VARIANT_AUTO) -> torch.Tensor:
     """Slices a bilateral grid with a guide image (reference op ``BilateralSlice``,
@@ -203,31 +264,10 @@ def bilateral_slice_apply(grid: torch.Tensor, guide: torch.Tensor, input: torch.
     ``variant`` forces a kernel variant for tests."""
     del name
     lib = _lib.load()
-    grid = _f32c(grid, "grid")
-    guide = _f32c(guide, "guide")
-    input = _f32c(input, "input")  # noqa: A001
-    if grid.dim() != 5:
-        raise ValueError("Input grid should be 5D (batch_size, height, width, depth, "
-                         "output_channels * input_channels)")
-    if guide.dim() != 3:
-        raise ValueError("Guide image should be 3D (batch_size, height, width)")
-    if input.dim() != 4:
-        raise ValueError("Input image should be 4D (batch_size, height, width, input_channels)")
-    if tuple(input.shape[:3]) != tuple(guide.shape):
-        raise ValueError("Input and guide size should match.")
-    if guide.shape[0] != grid.shape[0]:
-        raise ValueError("Batch sizes should match.")
     has_offset = bool(has_offset)
-    B, gh, gw, gd, gc = grid.shape
+    grid, guide, input, n_out = _slice_apply_args(grid, guide, input, has_offset)  # noqa: A001
+    B, gh, gw, gd, _ = grid.shape
     _, H, W, n_in = input.shape
-    J = n_in + (1 if has_offset else 0)
-    if gc % J != 0:
-        if has_offset:
-            raise ValueError("Slicing with affine offset, grid should have "
-                             "output_channels * (input_channels + 1) channels.")
-        raise ValueError("Slicing without affine offset, grid should have "
-                         "output_channels * input_channels channels.")
-    n_out = gc // J
     dev = _same_device(grid, guide, input)
     _require_cuda()
 
@@ -237,28 +277,12 @@ def bilateral_slice_apply(grid: torch.Tensor, guide: torch.Tensor, input: torch.
                 or not out.is_contiguous():
             raise ValueError(f"out must be a contiguous float32 tensor of shape {shape} on {dev}")
 
-    if dev.type == "cuda" and out is None and _wants_grad(grid, guide, input):
-        return _SliceApplyFn.apply(grid, guide, input, has_offset)
-
     if dev.type == "cuda":
         if out is None:
+            if _wants_grad(grid, guide, input):
+                return _SliceApplyFn.apply(grid, guide, input, has_offset)
             out = torch.empty(shape, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            # A workspace from torch's caching allocator (the library never allocates) lets AUTO
-            # pick the texture-assisted kernel for large images (>= 2 Mi px, W % 4 == 0).
-            ws_ptr, ws_bytes = 0, 0
-            explicit_tex = int(variant) in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
-            if (int(variant) == _lib.VARIANT_AUTO or explicit_tex) and n_in == 3 and n_out == 3 \
-                    and has_offset and W % 4 == 0 and \
-                    (explicit_tex or _texture_form_runs(dev.index, B, H, W, gh, gw, gd)):
-                ws = _workspace(dev, lib.hdrnet_slice_apply_workspace_bytes(B, H, gw, gd))
-                ws_ptr, ws_bytes = ws.data_ptr(), ws.numel() * 4
-            rc = lib.hdrnet_slice_apply_f32_ws(
-                grid.data_ptr(), guide.data_ptr(), input.data_ptr(), out.data_ptr(), B, H, W, gh,
-                gw, gd, n_in, n_out, int(has_offset), int(variant), ws_ptr, ws_bytes, stream)
-        _lib.check(rc, "BilateralSliceApply")
-        return out
+        return _launch_slice_apply(grid, guide, input, out, H, 0, n_out, has_offset, variant, "BilateralSliceApply")
 
     # Host buffers: pipelined copies + kernels on the current CUDA device.
     if out is None:
@@ -285,33 +309,10 @@ def bilateral_slice_apply_rows(grid: torch.Tensor, guide: torch.Tensor, input: t
     need no halo and equal the rows of the whole-image call bit for bit (same kernel).  Beyond the
     reference: it is the multi-GPU fallback for fewer images than GPUs (SURVEY.md section 8e,
     ``parallel.slice_apply_sharded``).  Inference only (no gradient registration); CUDA tensors."""
-    lib = _lib.load()
-    grid = _f32c(grid, "grid")
-    guide = _f32c(guide, "guide")
-    input = _f32c(input, "input")  # noqa: A001
-    if grid.dim() != 5:
-        raise ValueError("Input grid should be 5D (batch_size, height, width, depth, "
-                         "output_channels * input_channels)")
-    if guide.dim() != 3:
-        raise ValueError("Guide image should be 3D (batch_size, height, width)")
-    if input.dim() != 4:
-        raise ValueError("Input image should be 4D (batch_size, height, width, input_channels)")
-    if tuple(input.shape[:3]) != tuple(guide.shape):
-        raise ValueError("Input and guide size should match.")
-    if guide.shape[0] != grid.shape[0]:
-        raise ValueError("Batch sizes should match.")
-    has_offset = bool(has_offset)
-    B, gh, gw, gd, gc = grid.shape
-    _, rows, W, n_in = input.shape
-    y_off, height = int(y_off), int(height)
-    if y_off < 0 or y_off + rows > height:
-        raise ValueError(f"row band [{y_off}, {y_off + rows}) does not fit an image of {height} rows")
-    J = n_in + (1 if has_offset else 0)
-    if gc % J != 0:
-        raise ValueError("Slicing with affine offset, grid should have output_channels * (input_channels + 1) "
-                         "channels." if has_offset else
-                         "Slicing without affine offset, grid should have output_channels * input_channels channels.")
-    n_out = gc // J
+    _lib.load()
+    has_offset, y_off, height = bool(has_offset), int(y_off), int(height)
+    grid, guide, input, n_out = _slice_apply_args(grid, guide, input, has_offset, (y_off, height))  # noqa: A001
+    B, rows, W, _ = input.shape
     dev = _same_device(grid, guide, input)
     _require_cuda()
     if dev.type != "cuda":
@@ -324,20 +325,8 @@ def bilateral_slice_apply_rows(grid: torch.Tensor, guide: torch.Tensor, input: t
         out = torch.empty(shape, dtype=torch.float32, device=dev)
     elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != dev or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous float32 tensor of shape {shape} on {dev}")
-    with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        ws_ptr, ws_bytes = 0, 0
-        explicit_tex = int(variant) in (_lib.VARIANT_TEX, _lib.VARIANT_TEX_ASYNC)
-        if (int(variant) == _lib.VARIANT_AUTO or explicit_tex) and n_in == 3 and n_out == 3 \
-                and has_offset and W % 4 == 0 and \
-                (explicit_tex or _texture_form_runs(dev.index, B, rows, W, gh, gw, gd)):
-            ws = _workspace(dev, lib.hdrnet_slice_apply_workspace_bytes(B, rows, gw, gd))
-            ws_ptr, ws_bytes = ws.data_ptr(), ws.numel() * 4
-        rc = lib.hdrnet_slice_apply_rows_f32_ws(
-            grid.data_ptr(), guide.data_ptr(), input.data_ptr(), out.data_ptr(), B, height, W, rows, y_off,
-            gh, gw, gd, n_in, n_out, int(has_offset), int(variant), ws_ptr, ws_bytes, stream)
-    _lib.check(rc, "BilateralSliceApply(rows)")
-    return out
+    return _launch_slice_apply(grid, guide, input, out, height, y_off, n_out, has_offset, variant,
+                               "BilateralSliceApply(rows)")
 
 
 def slice_indices(guide: torch.Tensor, grid_shape) -> torch.Tensor:

@@ -35,19 +35,12 @@ def relu(x: torch.Tensor) -> torch.Tensor:
 
 
 def _layer_variables(scope, weights, use_bias, batch_norm, device):
-    """(weights, bias-or-None) on `device`, inference batch norm folded in (models._fold)."""
+    """(weights, bias-or-None) on `device`, as the models prepare a layer (models._layer_weights)."""
     from . import models
     if scope is None:
         raise ValueError("scope is required: it names the layer's variables (<scope>/weights, ...)")
     wts = weights if weights is not None else models._resolve_weights({})
-    if not batch_norm and isinstance(wts.get(scope + "/weights"), torch.Tensor):
-        # tensor variables are used as they are, so that gradients reach them
-        wd = models._device_var(wts[scope + "/weights"], device)
-        return wd, (models._device_var(wts[scope + "/biases"], device) if use_bias else None)
-    host = models._HostView(wts) if models._has_tensors(wts) else wts
-    w, b = models._fold(host, scope, bool(batch_norm), bool(use_bias))
-    wd = torch.from_numpy(w).contiguous().to(device)
-    return wd, (None if b is None else torch.from_numpy(b).contiguous().to(device))
+    return models._layer_weights(wts, scope, bool(batch_norm), bool(use_bias), device)
 
 
 def _refuse_batch_norm(scope, weights, batch_norm) -> None:

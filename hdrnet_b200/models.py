@@ -51,6 +51,7 @@ import numpy as np
 import torch
 
 from . import _lib, layers
+from .hdrnet_ops import _slice_apply_workspace, _workspace
 from .layers import bilateral_slice_apply
 
 __all__ = ["HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN", "set_weights", "load_weights",
@@ -194,32 +195,31 @@ def invalidate_prepared() -> None:
 def _fold(wts, scope, use_bn, use_bias):
     """Returns (weights, bias-or-None) as float32 numpy with inference batch norm folded in:
     y = (conv - mean) / sqrt(var + eps) + beta  (center=True, scale=False; layers.py:47-54;
-    the fold freeze_graph.py:141-142 applies)."""
-    w = np.asarray(wts[scope + "/weights"], np.float32)
+    the fold freeze_graph.py:141-142 applies).  Tensor variables are read through host copies."""
+    def var(name, dtype):
+        return np.asarray(_host(wts[f"{scope}/{name}"]), dtype)
+
+    w = var("weights", np.float32)
     if use_bn:
-        s = 1.0 / np.sqrt(np.asarray(wts[scope + "/BatchNorm/moving_variance"], np.float64) + BN_EPS)
-        b = np.asarray(wts[scope + "/BatchNorm/beta"], np.float64) - \
-            np.asarray(wts[scope + "/BatchNorm/moving_mean"], np.float64) * s
+        s = 1.0 / np.sqrt(var("BatchNorm/moving_variance", np.float64) + BN_EPS)
+        b = var("BatchNorm/beta", np.float64) - var("BatchNorm/moving_mean", np.float64) * s
         return (w.astype(np.float64) * s).astype(np.float32), b.astype(np.float32)
     if use_bias:
-        return w, np.asarray(wts[scope + "/biases"], np.float32)
+        return w, var("biases", np.float32)
     return w, None
+
+
+def _host(v):
+    """A variable as the host sees it: a tensor's detached host copy, anything else as it is."""
+    return v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v
+
+
+def _host_f32(v) -> np.ndarray:
+    return np.ascontiguousarray(_host(v), np.float32).reshape(-1)
 
 
 def _has_tensors(wts) -> bool:
     return any(isinstance(v, torch.Tensor) for v in wts.values())
-
-
-class _HostView:
-    """Read-only view of a weights dict with tensor values as host numpy arrays (for _fold and the
-    guide parameters, which the kernels take as host arrays)."""
-
-    def __init__(self, wts):
-        self._wts = wts
-
-    def __getitem__(self, key):
-        v = self._wts[key]
-        return v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v
 
 
 def _device_var(v, device) -> torch.Tensor:
@@ -243,48 +243,101 @@ def _coefficient_specs(params):
     return specs
 
 
+def _layer_weights(wts, scope, use_bn, use_bias, device):
+    """(weights, bias-or-None) of one layer as float32 tensors on `device`.  A batch-norm layer is
+    folded (_fold) into copies; any other layer runs on its variables as they are, so that a tensor
+    variable already on `device` is used without a copy and its gradient reaches it."""
+    if use_bn:
+        w, b = _fold(wts, scope, True, False)
+    else:
+        w, b = wts[scope + "/weights"], (wts[scope + "/biases"] if use_bias else None)
+    return _device_var(w, device), (None if b is None else _device_var(b, device))
+
+
+_CURVES_VARS = ("ccm", "ccm_bias", "shifts", "slopes", "channel_mixing/weights", "channel_mixing/biases")
+
+
+class _CurvesGuide:
+    """The curves guide (hdrnet/models.py:145-190) as its kernels take it: float32 host arrays ccm
+    [3, 3] ([in][out]), ccm_bias [3], shifts and slopes [3, 16], mix [3], the float mix_bias, and
+    `args`, the trailing arguments of hdrnet_guide_curves_f32 and hdrnet_slice_apply_curves_px_ws
+    (host pointers into the arrays this object keeps)."""
+
+    def __init__(self, ccm, ccm_bias, shifts, slopes, mix, mix_bias):
+        self.ccm = _host_f32(ccm).reshape(3, 3)
+        self.ccm_bias = _host_f32(ccm_bias).reshape(3)
+        self.shifts = _host_f32(shifts).reshape(3, 16)
+        self.slopes = _host_f32(slopes).reshape(3, 16)
+        self.mix = _host_f32(mix).reshape(3)
+        self.mix_bias = float(_host_f32(mix_bias)[0])
+        arrays = (self.ccm, self.ccm_bias, self.shifts, self.slopes, self.mix)
+        self.args = (*[_hp(a) for a in arrays], self.mix_bias)
+
+    @classmethod
+    def from_weights(cls, wts):
+        return cls(*[wts["inference/guide/" + n] for n in _CURVES_VARS])
+
+    def run(self, x: torch.Tensor) -> torch.Tensor:
+        """The standalone guide kernel over x [B, H, W, 3] (float32, contiguous) -> [B, H, W]."""
+        B, H, W, _ = x.shape
+        guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device):
+            rc = _lib.load().hdrnet_guide_curves_f32(x.data_ptr(), guide.data_ptr(), B * H * W, *self.args,
+                                                     _stream(x.device))
+        _lib.check(rc, "guide_curves")
+        return guide
+
+
+class _NNGuide:
+    """The pointwise-NN guide (hdrnet/models.py:199-210) with conv1's batch norm folded in: float32
+    host arrays w1 [3, F], b1 [F], w2 [F], the float b2 and the int feats F, and `args`, the trailing
+    arguments of hdrnet_guide_nn_f32 and hdrnet_slice_apply_nn_px_ws."""
+
+    def __init__(self, w1, b1, w2, b2):
+        self.w1 = _host_f32(w1).reshape(3, -1)
+        self.b1 = _host_f32(b1)
+        self.w2 = _host_f32(w2)
+        self.b2 = float(_host_f32(b2)[0])
+        self.feats = int(self.w1.shape[1])
+        self.args = (_hp(self.w1), _hp(self.b1), _hp(self.w2), self.b2, self.feats)
+
+    @classmethod
+    def folded(cls, wts, scope):
+        """The inference form: conv1's batch norm folded from the moving averages."""
+        w1, b1 = _fold(wts, scope + "/conv1", True, False)
+        return cls(w1, b1, wts[scope + "/conv2/weights"], wts[scope + "/conv2/biases"])
+
+    def run(self, x: torch.Tensor) -> torch.Tensor:
+        """The standalone guide kernel over x [B, H, W, 3] (float32, contiguous) -> [B, H, W]."""
+        B, H, W, _ = x.shape
+        guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device):
+            rc = _lib.load().hdrnet_guide_nn_f32(x.data_ptr(), guide.data_ptr(), B * H * W, *self.args,
+                                                 _stream(x.device))
+        _lib.check(rc, "guide_nn")
+        return guide
+
+
 class _Prepared:
-    """Device copies of the coefficient-network weights + host copies of the guide params."""
+    """Device copies of the coefficient-network weights + the guide's host parameters: `guides`, one
+    _CurvesGuide or _NNGuide, or one _NNGuide per level of the pyramid model."""
 
     def __init__(self, wts, params, device, nn_guide):
         self.device = device
         self.source = wts   # keeps the dict alive: the cache is keyed by id(wts)
         self.layers = {}
-        tensors = _has_tensors(wts)
-        host = _HostView(wts) if tensors else wts
         for scope, use_bn, use_bias in _coefficient_specs(params):
-            if tensors and not use_bn:
-                # the variables themselves (no copy when they are CUDA float32 already)
-                wd = _device_var(wts[scope + "/weights"], device)
-                bd = _device_var(wts[scope + "/biases"], device) if use_bias else None
-            else:
-                w, b = _fold(host, scope, use_bn, use_bias)
-                wd = torch.from_numpy(np.ascontiguousarray(w)).to(device)
-                bd = None if b is None else torch.from_numpy(np.ascontiguousarray(b)).to(device)
+            wd, bd = _layer_weights(wts, scope, use_bn, use_bias, device)
             # tensor variables change between optimizer steps: packed per call (this object is)
             packed = pack_conv_weights(wd.detach()) if (wd.dim() == 4 and device.type == "cuda") else None
             self.layers[scope] = (wd, bd, packed)
-        wts = host
         g = "inference/guide"
-        f32 = lambda a: np.ascontiguousarray(np.asarray(a, np.float32))  # noqa: E731
-
-        def nn_params(scope):
-            w1, b1 = _fold(wts, scope + "/conv1", True, False)
-            w1 = f32(w1.reshape(3, -1))
-            return (w1, f32(b1), f32(np.asarray(wts[scope + "/conv2/weights"]).reshape(-1)),
-                    float(np.asarray(wts[scope + "/conv2/biases"]).reshape(-1)[0]), int(w1.shape[1]))
-
         if nn_guide == "pyramid":     # HDRNetGaussianPyrNN: one pointwise NN per level
-            self.nn_levels = [nn_params(f"{g}/level_{lvl}") for lvl in range(3)]
+            self.guides = [_NNGuide.folded(wts, f"{g}/level_{lvl}") for lvl in range(3)]
         elif nn_guide:
-            self.nn_w1, self.nn_b1, self.nn_w2, self.nn_b2, self.nn_feats = nn_params(g)
+            self.guides = [_NNGuide.folded(wts, g)]
         else:
-            self.ccm = f32(wts[g + "/ccm"])
-            self.ccm_bias = f32(wts[g + "/ccm_bias"])
-            self.shifts = f32(np.asarray(wts[g + "/shifts"]).reshape(3, 16))
-            self.slopes = f32(np.asarray(wts[g + "/slopes"]).reshape(3, 16))
-            self.mix = f32(np.asarray(wts[g + "/channel_mixing/weights"]).reshape(3))
-            self.mix_bias = float(np.asarray(wts[g + "/channel_mixing/biases"]).reshape(-1)[0])
+            self.guides = [_CurvesGuide.from_weights(wts)]
 
 
 def _prepare(wts, params, device, nn_guide) -> _Prepared:
@@ -340,6 +393,30 @@ def _fused_row_kernel_takes(W: int, *bufs: torch.Tensor) -> bool:
     runs the guide kernel into the caller's buffer first.  A contiguous view at an offset (a frame
     carved out of a packed buffer, an ``out`` from a pool) is not aligned."""
     return W % 4 == 0 and W >= 128 and all(t.data_ptr() % 16 == 0 for t in bufs)
+
+
+def _slice_apply_fused(coeffs, x, guide, out_dtype, want_guide: bool, lend_workspace: bool):
+    """Guide + slice + apply in one kernel (hdrnet_slice_apply_{curves,nn}_px_ws): x [B,H,W,3]
+    (uint8 / uint16 / float32, contiguous), the coefficients [B,gh,gw,gd,3,4] and a _CurvesGuide or
+    _NNGuide -> (out [B,H,W,3] of `out_dtype`, the guide map [B,H,W] or None).  The map is written
+    when `want_guide` asks for it, and always where the float32 form runs the guide kernel into it
+    first (_fused_row_kernel_takes).  `lend_workspace`: lend the slab workspace with which AUTO runs
+    the texture-assisted kernel on large images."""
+    B, H, W, _ = x.shape
+    _, gh, gw, gd = coeffs.shape[:4]
+    in_fmt, out_fmt = _PX_FMT[x.dtype], _PX_FMT[out_dtype]
+    out = torch.empty((B, H, W, 3), dtype=out_dtype, device=x.device)
+    f32 = in_fmt == _lib.PX_F32 and out_fmt == _lib.PX_F32
+    gmap = torch.empty((B, H, W), dtype=torch.float32, device=x.device) \
+        if want_guide or (f32 and not _fused_row_kernel_takes(W, x, out, coeffs)) else None
+    lib = _lib.load()
+    launch = lib.hdrnet_slice_apply_nn_px_ws if isinstance(guide, _NNGuide) else lib.hdrnet_slice_apply_curves_px_ws
+    with torch.cuda.device(x.device):
+        ws = _slice_apply_workspace(x.device, B, H, W, gh, gw, gd) if lend_workspace else None
+        rc = launch(coeffs.data_ptr(), x.data_ptr(), in_fmt, out.data_ptr(), out_fmt, _ptr(gmap), B, H, W,
+                    gh, gw, gd, *guide.args, _ptr(ws), 0 if ws is None else ws.numel() * 4, _stream(x.device))
+    _lib.check(rc, "BilateralSliceApply(fused guide)")
+    return out, gmap
 
 
 def lowres_from_image(image: torch.Tensor, size: int) -> torch.Tensor:
@@ -438,11 +515,6 @@ def _stream(device):
     return torch.cuda.current_stream(device).cuda_stream
 
 
-def _grad_workspace(device, nbytes: int) -> torch.Tensor:
-    """Partial-sum workspace of one VJP call, lent to the library (it never allocates)."""
-    return torch.empty((max(int(nbytes), 16) + 3) // 4, dtype=torch.float32, device=device)
-
-
 def _ptr(t) -> int:
     return 0 if t is None else t.data_ptr()
 
@@ -482,7 +554,7 @@ class _ConvFn(torch.autograd.Function):
         lib = _lib.load()
         ws = None
         if dw is not None or db is not None:
-            ws = _grad_workspace(x.device, lib.hdrnet_conv2d_grad_workspace_bytes(B, H, W, cin, cout, k, ctx.stride))
+            ws = _workspace(x.device, lib.hdrnet_conv2d_grad_workspace_bytes(B, H, W, cin, cout, k, ctx.stride))
         with torch.cuda.device(x.device):
             rc = lib.hdrnet_conv2d_grad_f32(
                 x.data_ptr(), w.data_ptr(), out.data_ptr(), dy.data_ptr(), _ptr(dx), _ptr(dw), _ptr(db),
@@ -523,7 +595,7 @@ class _FcFn(torch.autograd.Function):
         lib = _lib.load()
         ws = None
         if dw is not None or db is not None:
-            ws = _grad_workspace(x.device, lib.hdrnet_fc_grad_workspace_bytes(B, I, O))
+            ws = _workspace(x.device, lib.hdrnet_fc_grad_workspace_bytes(B, I, O))
         with torch.cuda.device(x.device):
             rc = lib.hdrnet_fc_grad_f32(
                 x.data_ptr(), w.data_ptr(), out.data_ptr(), dy.data_ptr(), _ptr(dx), _ptr(dw), _ptr(db),
@@ -572,7 +644,7 @@ class _FusePredictFn(torch.autograd.Function):
         lib = _lib.load()
         ws = None
         if dw is not None or db is not None:
-            ws = _grad_workspace(local.device, lib.hdrnet_fuse_predict_grad_workspace_bytes(
+            ws = _workspace(local.device, lib.hdrnet_fuse_predict_grad_workspace_bytes(
                 bs, gh, gw, C, gd, n_out, n_in))
         with torch.cuda.device(local.device):
             rc = lib.hdrnet_fuse_predict_grad_f32(
@@ -583,14 +655,21 @@ class _FusePredictFn(torch.autograd.Function):
         return dl, dg, dw, db, None, None, None
 
 
-_CURVES_VARS = ("ccm", "ccm_bias", "shifts", "slopes", "channel_mixing/weights", "channel_mixing/biases")
 # [start, end) of each variable in the library's 112-float parameter gradient (include/hdrnet_b200.h)
 _CURVES_GRAD_SLICES = ((0, 9), (9, 12), (12, 60), (60, 108), (108, 111), (111, 112))
 
 
-def _host_f32(v) -> np.ndarray:
-    a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
-    return np.ascontiguousarray(a, np.float32).reshape(-1)
+def _var_shapes(variables):
+    """(shape, device) of each tensor variable, None for the others: what _split_param_grad needs."""
+    return [(v.shape, v.device) if isinstance(v, torch.Tensor) else None for v in variables]
+
+
+def _split_param_grad(dp, needs, shapes, slices):
+    """The gradient of each variable out of a guide VJP's flat parameter gradient `dp`: [start, end)
+    in `slices`, None where it is not needed or the variable is no tensor.  A copy per variable:
+    optimizers may update a .grad in place."""
+    return [dp[a:b].reshape(s[0]).to(s[1], copy=True) if need and s is not None else None
+            for need, s, (a, b) in zip(needs, shapes, slices)]
 
 
 class _CurvesGuideFn(torch.autograd.Function):
@@ -601,19 +680,10 @@ class _CurvesGuideFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, ccm, ccm_bias, shifts, slopes, mix, mix_bias):
         x = x.contiguous()
-        host = [_host_f32(v) for v in (ccm, ccm_bias, shifts, slopes, mix, mix_bias)]
-        B, H, W, _ = x.shape
-        guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            rc = _lib.load().hdrnet_guide_curves_f32(
-                x.data_ptr(), guide.data_ptr(), B * H * W, *[_hp(a) for a in host[:5]], float(host[5][0]),
-                _stream(x.device))
-        _lib.check(rc, "guide_curves")
+        ctx.guide = _CurvesGuide(ccm, ccm_bias, shifts, slopes, mix, mix_bias)
         ctx.save_for_backward(x)
-        ctx.host = host
-        ctx.vars = [(v.shape, v.device) if isinstance(v, torch.Tensor) else None
-                    for v in (ccm, ccm_bias, shifts, slopes, mix, mix_bias)]
-        return guide
+        ctx.vars = _var_shapes((ccm, ccm_bias, shifts, slopes, mix, mix_bias))
+        return ctx.guide.run(x)
 
     @staticmethod
     def backward(ctx, dguide):
@@ -626,37 +696,32 @@ class _CurvesGuideFn(torch.autograd.Function):
         dx = torch.empty_like(x) if need_x else None
         dp = torch.empty(112, dtype=torch.float32, device=x.device) if need_p else None
         lib = _lib.load()
-        ws = _grad_workspace(x.device, lib.hdrnet_guide_curves_grad_workspace_bytes(npix)) if need_p else None
-        host = ctx.host
+        ws = _workspace(x.device, lib.hdrnet_guide_curves_grad_workspace_bytes(npix)) if need_p else None
         with torch.cuda.device(x.device):
             rc = lib.hdrnet_guide_curves_grad_f32(
-                x.data_ptr(), dguide.data_ptr(), _ptr(dx), npix, *[_hp(a) for a in host[:5]], float(host[5][0]),
+                x.data_ptr(), dguide.data_ptr(), _ptr(dx), npix, *ctx.guide.args,
                 _ptr(dp), _ptr(ws), 0 if ws is None else ws.numel() * 4, _stream(x.device))
         _lib.check(rc, "guide_curves VJP")
-        grads = []
-        for need, var, (a, b) in zip(ctx.needs_input_grad[1:], ctx.vars, _CURVES_GRAD_SLICES):
-            # a copy per variable: optimizers may update a .grad in place
-            grads.append(dp[a:b].reshape(var[0]).to(var[1], copy=True) if need and var is not None else None)
-        return (dx, *grads)
-
-
-def _curves_guide_grad(wts, params, x) -> bool:
-    """Whether HDRNetCurves._guide goes through autograd: grad enabled, params['guide_grad'] truthy,
-    and a guide variable or the input requiring grad."""
-    if not (torch.is_grad_enabled() and isinstance(params, dict) and params.get("guide_grad")):
-        return False
-    return _requires_grad(x) or (wts is not None and
-                                 any(_requires_grad(wts.get("inference/guide/" + n)) for n in _CURVES_VARS))
+        return (dx, *_split_param_grad(dp, ctx.needs_input_grad[1:], ctx.vars, _CURVES_GRAD_SLICES))
 
 
 _NN_GUIDE_VARS = ("conv1/weights", "conv1/BatchNorm/beta", "conv2/weights", "conv2/biases")
 _NN_MOVING = ("conv1/BatchNorm/moving_mean", "conv1/BatchNorm/moving_variance")
 
 
-class _BatchStats(collections.namedtuple("_BatchStats", "npix moments w1f b1f mean var host")):
+def _guide_grad(wts, params, x, names) -> bool:
+    """Whether a guide goes through autograd: grad enabled, params['guide_grad'] truthy, and the input
+    or one of the guide's variables `names` (under inference/guide/) requiring grad."""
+    if not (torch.is_grad_enabled() and isinstance(params, dict) and params.get("guide_grad")):
+        return False
+    return _requires_grad(x) or (wts is not None and
+                                 any(_requires_grad(wts.get("inference/guide/" + n)) for n in names))
+
+
+class _BatchStats(collections.namedtuple("_BatchStats", "npix moments guide mean var host")):
     """conv1's batch statistics of one training-mode call: the input's moments (float64 [9]), the
-    folded float32 weights the guide kernel runs with, the features' batch mean and biased variance
-    (float64), and the host copies (_host_f32) of the four variables they were folded from."""
+    _NNGuide on the folded weights the guide kernel runs with, the features' batch mean and biased
+    variance (float64), and the host copies (_host_f32) of the four variables they were folded from."""
 
 
 def _nn_batch_stats(x, host) -> _BatchStats:
@@ -667,7 +732,7 @@ def _nn_batch_stats(x, host) -> _BatchStats:
     w1, beta = host[0], host[1]
     feats = beta.size
     moments = torch.empty(9, dtype=torch.float64, device=x.device)
-    ws = _grad_workspace(x.device, lib.hdrnet_guide_nn_stats_workspace_bytes(npix))
+    ws = _workspace(x.device, lib.hdrnet_guide_nn_stats_workspace_bytes(npix))
     rc = lib.hdrnet_guide_nn_stats_f32(x.data_ptr(), npix, moments.data_ptr(), ws.data_ptr(), ws.numel() * 4,
                                        _stream(x.device))
     _lib.check(rc, "guide_nn batch statistics")
@@ -676,7 +741,7 @@ def _nn_batch_stats(x, host) -> _BatchStats:
     mean, var = np.empty(feats, np.float64), np.empty(feats, np.float64)
     rc = lib.hdrnet_guide_nn_batch_fold(_hp(w1), _hp(beta), _hp(mom), feats, _hp(w1f), _hp(b1f), _hp(mean), _hp(var))
     _lib.check(rc, "guide_nn batch-norm fold")
-    return _BatchStats(npix, mom, w1f, b1f, mean, var, host)
+    return _BatchStats(npix, mom, _NNGuide(w1f, b1f, host[2], host[3]), mean, var, host)
 
 
 def _update_moving_averages(moving, stats: _BatchStats) -> None:
@@ -708,16 +773,6 @@ def _moving_averages(wts):
     return out
 
 
-def _launch_nn_guide(x, w1, b1, w2, b2, feats) -> torch.Tensor:
-    """hdrnet_guide_nn_f32 with host weights (conv1's batch norm already folded) -> [B, H, W]."""
-    B, H, W, _ = x.shape
-    guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
-    rc = _lib.load().hdrnet_guide_nn_f32(x.data_ptr(), guide.data_ptr(), B * H * W, _hp(w1), _hp(b1), _hp(w2),
-                                         float(b2), int(feats), _stream(x.device))
-    _lib.check(rc, "guide_nn")
-    return guide
-
-
 class _NNGuideFn(torch.autograd.Function):
     """The pointwise-NN guide in training mode (hdrnet/models.py:203-210, batch norm with the batch's
     statistics) over x and its four variables (_NN_GUIDE_VARS order); `stats` is _nn_batch_stats of
@@ -727,12 +782,10 @@ class _NNGuideFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w1, beta, w2, b2, stats):
         x = x.contiguous()
-        host = stats.host
-        guide = _launch_nn_guide(x, stats.w1f, stats.b1f, host[2], host[3][0], host[1].size)
         ctx.save_for_backward(x)
         ctx.stats = stats
-        ctx.vars = [(v.shape, v.device) if isinstance(v, torch.Tensor) else None for v in (w1, beta, w2, b2)]
-        return guide
+        ctx.vars = _var_shapes((w1, beta, w2, b2))
+        return stats.guide.run(x)
 
     @staticmethod
     def backward(ctx, dguide):
@@ -747,25 +800,14 @@ class _NNGuideFn(torch.autograd.Function):
         dx = torch.empty_like(x) if need_x else None
         dp = torch.empty(5 * F + 1, dtype=torch.float32, device=x.device) if need_p else None
         lib = _lib.load()
-        ws = _grad_workspace(x.device, lib.hdrnet_guide_nn_grad_workspace_bytes(npix, F))
+        ws = _workspace(x.device, lib.hdrnet_guide_nn_grad_workspace_bytes(npix, F))
         with torch.cuda.device(x.device):
             rc = lib.hdrnet_guide_nn_grad_f32(
                 x.data_ptr(), dguide.data_ptr(), _ptr(dx), npix, _hp(w1), _hp(beta), _hp(w2), float(b2[0]), F,
                 _hp(st.moments), _ptr(dp), ws.data_ptr(), ws.numel() * 4, _stream(x.device))
         _lib.check(rc, "guide_nn VJP")
-        grads = []
         slices = ((0, 3 * F), (3 * F, 4 * F), (4 * F, 5 * F), (5 * F, 5 * F + 1))
-        for need, var, (a, b) in zip(ctx.needs_input_grad[1:5], ctx.vars, slices):
-            grads.append(dp[a:b].reshape(var[0]).to(var[1], copy=True) if need and var is not None else None)
-        return (dx, *grads, None)
-
-
-def _nn_guide_grad(wts, params, x) -> bool:
-    """Whether the training-mode pointwise-NN guide goes through autograd: grad enabled,
-    params['guide_grad'] truthy, and a guide variable or the input requiring grad."""
-    if not (torch.is_grad_enabled() and isinstance(params, dict) and params.get("guide_grad")):
-        return False
-    return _requires_grad(x) or any(_requires_grad(wts.get("inference/guide/" + n)) for n in _NN_GUIDE_VARS)
+        return (dx, *_split_param_grad(dp, ctx.needs_input_grad[1:5], ctx.vars, slices), None)
 
 
 def _requires_grad(t) -> bool:
@@ -859,11 +901,8 @@ class HDRNetCurves(object):
         _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=bool(cls._nn_guide))
         fullres_input = _check_input(fullres_input, "fullres_input")
         coeffs = cls._coefficients(lowres_input, params, is_training)
-        if coeffs.requires_grad or (not cls._nn_guide and _curves_guide_grad(wts, params, fullres_input)):
-            with torch.cuda.device(fullres_input.device):
-                guide = cls._guide(fullres_input, params)
-            B, gh, gw, gd = coeffs.shape[:4]
-            return bilateral_slice_apply(coeffs.reshape(B, gh, gw, gd, -1), guide, fullres_input, True)
+        if coeffs.requires_grad or (not cls._nn_guide and _guide_grad(wts, params, fullres_input, _CURVES_VARS)):
+            return cls._output(fullres_input, cls._guide(fullres_input, params), coeffs)
         return cls._fullres(coeffs, fullres_input, params, torch.float32)
 
     @classmethod
@@ -901,39 +940,8 @@ class HDRNetCurves(object):
     def _fullres(cls, coeffs, fullres_input, params, out_dtype):
         """Guide + slice + apply over the full-resolution image (models.py:53-58), one kernel."""
         prep = _prepare(_resolve_weights(params), params, fullres_input.device, cls._nn_guide)
-        B, H, W, _ = fullres_input.shape
-        _, gh, gw, gd = coeffs.shape[:4]
-        in_fmt, out_fmt = _PX_FMT[fullres_input.dtype], _PX_FMT[out_dtype]
-        out = torch.empty((B, H, W, 3), dtype=out_dtype, device=fullres_input.device)
         debug = bool(params.get("debug"))
-        f32 = in_fmt == _lib.PX_F32 and out_fmt == _lib.PX_F32
-        # the float32 form needs the guide buffer for shapes and buffers its row kernel cannot take
-        need_guide = debug or (f32 and not _fused_row_kernel_takes(W, fullres_input, out, coeffs))
-        guide = torch.empty((B, H, W), dtype=torch.float32, device=fullres_input.device) \
-            if need_guide else None
-        lib = _lib.load()
-        with torch.cuda.device(fullres_input.device):
-            stream = torch.cuda.current_stream(fullres_input.device).cuda_stream
-            gptr = 0 if guide is None else guide.data_ptr()
-            # workspace lent to the library (it never allocates): texture-assisted kernel for
-            # large images, exactly as hdrnet_ops.bilateral_slice_apply does
-            ws_ptr, ws_bytes = 0, 0
-            from .hdrnet_ops import _texture_form_runs, _workspace
-            if _texture_form_runs(fullres_input.device.index, B, H, W, gh, gw, gd):
-                ws = _workspace(fullres_input.device,
-                                lib.hdrnet_slice_apply_workspace_bytes(B, H, gw, gd))
-                ws_ptr, ws_bytes = ws.data_ptr(), ws.numel() * 4
-            if cls._nn_guide:
-                rc = lib.hdrnet_slice_apply_nn_px_ws(
-                    coeffs.data_ptr(), fullres_input.data_ptr(), in_fmt, out.data_ptr(), out_fmt,
-                    gptr, B, H, W, gh, gw, gd, _hp(prep.nn_w1), _hp(prep.nn_b1), _hp(prep.nn_w2),
-                    prep.nn_b2, prep.nn_feats, ws_ptr, ws_bytes, stream)
-            else:
-                rc = lib.hdrnet_slice_apply_curves_px_ws(
-                    coeffs.data_ptr(), fullres_input.data_ptr(), in_fmt, out.data_ptr(), out_fmt,
-                    gptr, B, H, W, gh, gw, gd, _hp(prep.ccm), _hp(prep.ccm_bias), _hp(prep.shifts),
-                    _hp(prep.slopes), _hp(prep.mix), prep.mix_bias, ws_ptr, ws_bytes, stream)
-        _lib.check(rc, "BilateralSliceApply(fused guide)")
+        out, guide = _slice_apply_fused(coeffs, fullres_input, prep.guides[0], out_dtype, debug, True)
         if debug:
             cls.last_debug = {"bilateral_coefficients": coeffs, "guide": guide, "output": out}
         return out
@@ -1017,22 +1025,13 @@ class HDRNetCurves(object):
     @classmethod
     def _guide(cls, input_tensor, params, is_training=False):
         """models.py:145-190 as a standalone kernel -> [B, H, W].  Differentiable (_CurvesGuideFn)
-        when _curves_guide_grad says so."""
+        when _guide_grad says so."""
         x = _check_input(input_tensor, "fullres_input")
         wts = _resolve_weights(params)
-        if _curves_guide_grad(wts, params, x):
+        if _guide_grad(wts, params, x, _CURVES_VARS):
             with torch.cuda.device(x.device):
                 return _CurvesGuideFn.apply(x, *[wts["inference/guide/" + n] for n in _CURVES_VARS])
-        prep = _prepare(wts, params, x.device, False)
-        B, H, W, _ = x.shape
-        guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            rc = _lib.load().hdrnet_guide_curves_f32(
-                x.data_ptr(), guide.data_ptr(), B * H * W, _hp(prep.ccm), _hp(prep.ccm_bias),
-                _hp(prep.shifts), _hp(prep.slopes), _hp(prep.mix), prep.mix_bias,
-                torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(rc, "guide_curves")
-        return guide
+        return _prepare(wts, params, x.device, False).guides[0].run(x)
 
     @classmethod
     def _output(cls, im, guide, coeffs):
@@ -1069,17 +1068,13 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
         _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True)
         fullres_input = _check_input(fullres_input, "fullres_input")
         coeffs = cls._coefficients(lowres_input, params)
-        with torch.cuda.device(fullres_input.device):
-            guide = cls._guide(fullres_input, params, is_training=True)
-        B, gh, gw, gd = coeffs.shape[:4]
-        return bilateral_slice_apply(coeffs.reshape(B, gh, gw, gd, -1), guide, fullres_input, True)
+        return cls._output(fullres_input, cls._guide(fullres_input, params, is_training=True), coeffs)
 
     @classmethod
     def _guide(cls, input_tensor, params, is_training=False):
         """models.py:199-210 -> [B, H, W].  Inference form: conv1's batch norm folded from the moving
         averages.  ``is_training=True``: normalised with the batch's statistics (_nn_batch_stats), the
-        moving averages updated in place, and differentiable (_NNGuideFn) when _nn_guide_grad says
-        so."""
+        moving averages updated in place, and differentiable (_NNGuideFn) when _guide_grad says so."""
         if is_training:
             wts = _resolve_weights(params)
             moving = _moving_averages(wts)
@@ -1088,25 +1083,15 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
             if x.numel() == 0:
                 raise ValueError("fullres_input is empty: batch statistics need at least one pixel")
             variables = [wts["inference/guide/" + n] for n in _NN_GUIDE_VARS]
-            host = [_host_f32(v) for v in variables]
             with torch.cuda.device(x.device):
                 x = x.contiguous()
-                stats = _nn_batch_stats(x, host)
+                stats = _nn_batch_stats(x, [_host_f32(v) for v in variables])
                 _update_moving_averages(moving, stats)
-                if _nn_guide_grad(wts, params, x):
+                if _guide_grad(wts, params, x, _NN_GUIDE_VARS):
                     return _NNGuideFn.apply(x, *variables, stats)
-                return _launch_nn_guide(x, stats.w1f, stats.b1f, host[2], host[3][0], host[1].size)
+                return stats.guide.run(x)
         x = _check_input(input_tensor, "fullres_input")
-        prep = _prepare(_resolve_weights(params), params, x.device, True)
-        B, H, W, _ = x.shape
-        guide = torch.empty((B, H, W), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            rc = _lib.load().hdrnet_guide_nn_f32(
-                x.data_ptr(), guide.data_ptr(), B * H * W, _hp(prep.nn_w1), _hp(prep.nn_b1),
-                _hp(prep.nn_w2), prep.nn_b2, prep.nn_feats,
-                torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(rc, "guide_nn")
-        return guide
+        return _prepare(_resolve_weights(params), params, x.device, True).guides[0].run(x)
 
 
 def _resize(x: torch.Tensor, oh: int, ow: int, add: torch.Tensor | None = None) -> torch.Tensor:
@@ -1184,17 +1169,7 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
     def _guide(cls, multiscale, params, is_training=False):
         """models.py:264-272: HDRNetPointwiseNNGuide._guide per level (scope level_{il})."""
         prep = _prepare(_resolve_weights(params), params, multiscale[0].device, "pyramid")
-        lib = _lib.load()
-        guides = []
-        for lvl, (w1, b1, w2, b2, feats) in zip(multiscale, prep.nn_levels):
-            B, H, W, _ = lvl.shape
-            g = torch.empty((B, H, W), dtype=torch.float32, device=lvl.device)
-            rc = lib.hdrnet_guide_nn_f32(lvl.data_ptr(), g.data_ptr(), B * H * W, _hp(w1), _hp(b1),
-                                         _hp(w2), b2, feats,
-                                         torch.cuda.current_stream(lvl.device).cuda_stream)
-            _lib.check(rc, "guide_nn")
-            guides.append(g)
-        return guides
+        return [guide.run(lvl) for lvl, guide in zip(multiscale, prep.guides)]
 
     @classmethod
     def _output(cls, lvls, guide_lvls, coeffs, params=None):
@@ -1202,7 +1177,6 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
         guide is computed inside its slice-apply kernel."""
         prep = _prepare(_resolve_weights(params), params, lvls[0].device, "pyramid") \
             if guide_lvls is None else None
-        lib = _lib.load()
         B, gh, gw, gd = coeffs.shape[:4]
         current = None
         for il in range(cls.n_scales()):
@@ -1213,16 +1187,7 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
             if guide_lvls is not None:
                 out_lvl = bilateral_slice_apply(c, guide_lvls[src], lvl, has_offset=True)
             else:
-                w1, b1, w2, b2, feats = prep.nn_levels[src]
-                out_lvl = torch.empty_like(lvl)
-                need_guide = not _fused_row_kernel_takes(W, lvl, out_lvl, c)
-                scratch = torch.empty((B, H, W), dtype=torch.float32, device=lvl.device) \
-                    if need_guide else None
-                rc = lib.hdrnet_slice_apply_nn_f32(
-                    c.data_ptr(), lvl.data_ptr(), out_lvl.data_ptr(),
-                    0 if scratch is None else scratch.data_ptr(), B, H, W, gh, gw, gd, _hp(w1),
-                    _hp(b1), _hp(w2), b2, feats, torch.cuda.current_stream(lvl.device).cuda_stream)
-                _lib.check(rc, "BilateralSliceApply(fused NN guide)")
+                out_lvl = _slice_apply_fused(c, lvl, prep.guides[src], torch.float32, False, False)[0]
             current = out_lvl if il == 0 else _resize(current, H, W, add=out_lvl)
         return current
 

@@ -140,7 +140,7 @@ def test_upgraded_legacy_weights_load_into_the_model():
 
 
 @pytest.mark.parametrize("model_name", ["HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN"])
-def test_guide_bins_layout_and_round_trip(tmp_path, model_name):
+def test_guide_bins_layout_and_round_trip_to_the_guide_objects(tmp_path, model_name):
     p = dict(M.DEFAULT_PARAMS, model_name=model_name, batch_norm=True)
     wts = models.init_weights(p, seed=2, model_name=model_name)
     paths = C.export_guide_bins(wts, model_name, str(tmp_path))
@@ -156,19 +156,19 @@ def test_guide_bins_layout_and_round_trip(tmp_path, model_name):
         assert np.array_equal(raw[:, :3], np.asarray(wts[f"{g}/ccm"]).T)              # [out][in | bias]
         assert np.array_equal(raw[:, 3], np.asarray(wts[f"{g}/ccm_bias"]))
         back = C.load_guide_bins(str(tmp_path), model_name)
-        prep = models._Prepared(wts, p, torch.device("cpu"), False)                                  # what the kernels get
+        (guide,) = models._Prepared(wts, p, torch.device("cpu"), False).guides                      # what the kernels get
         for k in ("ccm", "ccm_bias", "shifts", "slopes", "mix"):
-            assert np.array_equal(back[k], getattr(prep, k)), k
-        assert back["mix_bias"] == prep.mix_bias
+            assert np.array_equal(back[k], getattr(guide, k)), k
+        assert back["mix_bias"] == guide.mix_bias
     else:
         levels = [f"{g}/level_{l}" for l in range(3)] if model_name == "HDRNetGaussianPyrNN" else [g]
         assert len(names) == 2 * len(levels)
         back = C.load_guide_bins(str(tmp_path), model_name)
         prep = models._Prepared(wts, p, torch.device("cpu"), "pyramid" if len(levels) == 3 else True)
-        for l, scope in enumerate(levels):
+        assert len(prep.guides) == len(levels)
+        for l, (scope, guide) in enumerate(zip(levels, prep.guides)):
             b = back[f"level_{l}"] if len(levels) == 3 else back
-            w1, b1, w2, b2, feats = prep.nn_levels[l] if len(levels) == 3 else \
-                (prep.nn_w1, prep.nn_b1, prep.nn_w2, prep.nn_b2, prep.nn_feats)
+            w1, b1, w2, b2, feats = guide.w1, guide.b1, guide.w2, guide.b2, guide.feats
             assert feats == 16 and b["w1"].shape == (3, 16)
             # the freeze step folds in float32, the kernels' packer in float64: 1 ulp apart at most
             np.testing.assert_allclose(b["w1"], w1, rtol=3e-7, atol=0)

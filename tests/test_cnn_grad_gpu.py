@@ -304,6 +304,16 @@ def test_layers_conv_and_fc_with_tensor_variables():
     v = G.fc_vjp(np_(xf), np_(w[f + "/weights"]), np_(yf), dyf, False)
     assert rel(np_(xf.grad), v.dx) <= BAR
     check_wgrad("layers.fc dw", np_(w[f + "/weights"].grad), v.dw, v.dw_abs)
+    # numpy weights next to a bias tensor that requires grad: the bias is used as it is and gets its gradient
+    mixed = {k: np_(t) if k.endswith("/weights") else cuda(np_(t), True) for k, t in w.items()}
+    y = layers.conv(x.detach(), 16, 3, stride=2, scope=s, weights=mixed)
+    y.backward(cuda(dy))
+    v = G.conv_vjp(np_(x), mixed[s + "/weights"], np_(y), dy, 2, True)
+    check_wgrad("layers.conv db, numpy weights", np_(mixed[s + "/biases"].grad), v.db, v.db_abs)
+    yf = layers.fc(xf.detach(), 32, scope=f, weights=mixed, activation_fn=None)
+    yf.backward(cuda(dyf))
+    v = G.fc_vjp(np_(xf), mixed[f + "/weights"], np_(yf), dyf, False)
+    check_wgrad("layers.fc db, numpy weights", np_(mixed[f + "/biases"].grad), v.db, v.db_abs)
 
 
 @pytest.mark.parametrize("model", [models.HDRNetCurves, models.HDRNetPointwiseNNGuide])

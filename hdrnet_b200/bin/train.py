@@ -50,6 +50,23 @@ resize VJP are not implemented, so ``--batch_norm``, ``HDRNetGaussianPyrNN`` and
 with ``HDRNetPointwiseNNGuide`` without ``--guide_batch_stats`` are refused before any data is read,
 with the models' own ``NotImplementedError``.
 
+Data-parallel training on one host: ``torchrun --nproc-per-node N -m hdrnet_b200.bin.train ...``
+(``WORLD_SIZE`` > 1) runs one process per GPU, rank r on ``cuda:(LOCAL_RANK % device_count)``, and
+trains what one process with the same flags trains, up to the order of float32 sums.
+``--batch_size`` is the global batch, as in the reference; N must divide it (``ValueError`` before
+any data is read), and rank r builds rows ``[r B / N, (r + 1) B / N)`` of each batch on either data
+tier.  The initial variables are broadcast from rank 0.  After ``backward`` the gradients are
+averaged over the ranks with one all-reduce of a flat float32 buffer, so every rank takes the same
+Adam step; with ``--guide_batch_stats`` the guide's batch norm uses the whole batch's statistics
+(models merges the ranks' moments).  One small all-reduce per step averages the logged loss and PSNR
+and carries rank 0's decisions to evaluate and to checkpoint, so no rank decides from its own clock.
+Rank 0 alone logs, writes ``train_log.jsonl`` and writes the checkpoints (``on_stop.ckpt`` after an
+interrupt included); before each checkpoint the ranks compare a digest of their variables and Adam
+moments and raise if they have drifted apart.  The evaluation splits the eval set by index over the
+ranks.  The world size is not a model parameter and is not written to ``params.json``: a checkpoint
+resumes with any world size, since the batches depend only on ``(seed, step)`` and the global batch.
+Without ``WORLD_SIZE`` (or with 1) no process group is made and no collective runs.
+
 Deliberate differences from the reference:
 
 * ``--max_steps`` (the reference runs until interrupted), ``--seed``, ``--train_guide`` and
@@ -81,7 +98,9 @@ import time
 import numpy as np
 import torch
 
-from hdrnet_b200 import checkpoint, data_pipeline, metrics, models
+import torch.distributed as dist
+
+from hdrnet_b200 import checkpoint, data_pipeline, metrics, models, parallel
 
 logging.basicConfig(format="[%(process)d] %(levelname)s %(filename)s:%(lineno)s | %(message)s")
 log = logging.getLogger("train")
@@ -250,7 +269,12 @@ class Trainer:
         os.makedirs(args.checkpoint_dir, exist_ok=True)
         self.mdl = getattr(models, params["model_name"])
         self.device = torch.device("cuda", torch.cuda.current_device())
-        init = models.init_weights(params, seed=args.seed, model_name=params["model_name"])
+        self.world = parallel.world_size()
+        self.rank = dist.get_rank() if self.world > 1 else 0
+        if self.rank:
+            log.setLevel(logging.WARNING)           # rank 0 speaks for the run
+        init = parallel.broadcast_weights(models.init_weights(params, seed=args.seed,
+                                                              model_name=params["model_name"]))
         self.weights = {k: torch.from_numpy(v).to(self.device) for k, v in init.items()}
         self.names = trained_names(self.weights, args.train_guide)
         for k in self.names:
@@ -270,7 +294,8 @@ class Trainer:
         self.train_data = data_pipeline.ImageFilesDataPipeline(
             args.data_dir, batch_size=args.batch_size, output_resolution=args.output_resolution, shuffle=True,
             fliplr=args.fliplr, flipud=args.flipud, rotate=args.rotate, random_crop=args.random_crop,
-            params=params, nthreads=args.data_threads, seed=args.seed, device=self.device)
+            params=params, nthreads=args.data_threads, seed=args.seed, device=self.device,
+            shard=(self.rank, self.world))
         self.eval_data = None
         if args.eval_data_dir is not None:
             self.eval_data = data_pipeline.ImageFilesDataPipeline(
@@ -303,8 +328,11 @@ class Trainer:
         self.ema.update(ema)
         log.info("resumed %s at step %d", prefix, step)
 
-    def save(self, name=None):
-        """Write ``model.ckpt-<step>`` (or ``name``) and params.json; returns the prefix."""
+    def save(self, name=None, check_ranks=True):
+        """Write ``model.ckpt-<step>`` (or ``name``) and params.json; returns the prefix.  Under a
+        process group every rank calls it: with ``check_ranks`` the ranks first compare a digest of
+        their variables and Adam moments (RuntimeError when they have drifted apart), then rank 0
+        alone writes, since every rank holds the same state."""
         prefix = os.path.join(self.args.checkpoint_dir, name or f"model.ckpt-{self.step}")
         moments = {}
         for k in self.names:
@@ -312,6 +340,12 @@ class Trainer:
             zero = torch.zeros_like(self.weights[k])
             moments[k] = (st["exp_avg"] if st else zero).cpu().numpy(), (st["exp_avg_sq"] if st else zero).cpu().numpy()
         variables = {k: v.detach().cpu().numpy() for k, v in self.weights.items()}
+        if check_ranks:
+            parallel.check_ranks_agree([variables[k] for k in sorted(variables)]
+                                       + [a for k in self.names for a in moments[k]],
+                                       f"the variables and Adam moments at step {self.step}")
+        if self.rank:
+            return prefix
         checkpoint.write_tf_checkpoint(prefix, checkpoint_tensors(variables, moments, self.step, self.ema))
         with open(os.path.join(self.args.checkpoint_dir, "params.json"), "w") as f:
             json.dump(self.params, f)
@@ -320,7 +354,10 @@ class Trainer:
 
     # ---- steps ---------------------------------------------------------------------------------
     def train_step(self):
-        """One gradient step on batch ``self.step``; returns (loss, psnr) as device scalars."""
+        """One gradient step on batch ``self.step`` (this rank's shard of it); returns (loss, psnr)
+        over the shard as device scalars.  Under a process group the gradients are averaged over the
+        ranks (parallel.all_reduce_mean_, one all-reduce) before Adam, so every rank takes the step of
+        the whole batch's mean loss."""
         batch = self.train_data.batch(self.step)
         self.opt.zero_grad(set_to_none=True)
         pred = self.mdl.inference(batch["lowres_input"], batch["image_input"], self.p,
@@ -329,19 +366,25 @@ class Trainer:
         with torch.no_grad():
             psnr = metrics.psnr(batch["image_output"], pred)
         loss.backward()
+        if self.world > 1:
+            for k in self.names:
+                if self.weights[k].grad is None:
+                    self.weights[k].grad = torch.zeros_like(self.weights[k])
+            parallel.all_reduce_mean_([self.weights[k].grad for k in self.names])
         self.opt.step()
         self.step += 1
         return loss.detach(), psnr
 
     def evaluate(self) -> float:
-        """Mean PSNR over the eval set (batch 1, no augmentation, centre crop)."""
+        """Mean PSNR over the eval set (batch 1, no augmentation, centre crop).  Under a process group
+        rank r scores images r, r + world, ... and the sums are added over the ranks."""
         total = 0.0
         with torch.no_grad():
-            for i in range(self.eval_data.nsamples):
+            for i in range(self.rank, self.eval_data.nsamples, self.world):
                 b = self.eval_data.batch(i)
                 total += float(metrics.psnr(b["image_output"],
                                             self.mdl.inference(b["lowres_input"], b["image_input"], self.p)))
-        return total / self.eval_data.nsamples
+        return float(parallel.sum_over_ranks([total])[0]) / self.eval_data.nsamples
 
     def record(self, rec):
         with open(os.path.join(self.args.checkpoint_dir, "train_log.jsonl"), "a") as f:
@@ -357,38 +400,48 @@ class Trainer:
         a = self.args
         t0 = time.time()
         last_log = last_summary = last_ckpt = last_eval = t0
+        interrupted = False
         try:
             while a.max_steps is None or self.step < a.max_steps:
                 loss_t, psnr_t = self.train_step()
                 loss, psnr = float(loss_t), float(psnr_t)
+                now = time.time()
+                lead = self.rank == 0       # rank 0's clock decides what every rank does this step
+                evaluate = lead and self.eval_data is not None and now - last_eval >= a.eval_interval
+                save = lead and now - last_ckpt >= a.checkpoint_interval
+                if self.world > 1:          # one all-reduce: the shards' mean scalars and rank 0's decisions
+                    loss, psnr, evaluate, save = parallel.sum_over_ranks([loss, psnr, evaluate, save])
+                    loss, psnr, evaluate, save = loss / self.world, psnr / self.world, evaluate > 0, save > 0
                 for key, val in (("loss", loss), ("psnr", psnr)):
                     self.ema[key] = EMA_DECAY * self.ema[key] + (1.0 - EMA_DECAY) * val
                 debias = 1.0 - EMA_DECAY ** self.step
                 loss_ema, psnr_ema = self.ema["loss"] / debias, self.ema["psnr"] / debias
-                now = time.time()
-                if now - last_log >= a.log_interval:
+                if lead and now - last_log >= a.log_interval:
                     log.info("Step %d | loss = %.4f | psnr = %.1f dB", self.step, loss_ema, psnr_ema)
                     last_log = now
-                if now - last_summary >= a.summary_interval:
+                if lead and now - last_summary >= a.summary_interval:
                     self.record({"step": self.step, "time": now - t0, "loss": loss, "psnr": psnr,
                                  "loss_ema": loss_ema, "psnr_ema": psnr_ema,
                                  "learning_rate": a.learning_rate, "batch_size": a.batch_size})
                     last_summary = now
-                if self.eval_data is not None and now - last_eval >= a.eval_interval:
+                if evaluate:
                     log.info("Evaluating on %d images at step %d", self.eval_data.nsamples, self.step)
                     p = self.evaluate()
                     log.info("  Evaluation PSNR = %.1f dB", p)
-                    self.record({"step": self.step, "time": time.time() - t0, "eval_psnr": p})
+                    if lead:
+                        self.record({"step": self.step, "time": time.time() - t0, "eval_psnr": p})
                     last_eval = time.time()
-                if now - last_ckpt >= a.checkpoint_interval:
+                if save:
                     self.save()
                     last_ckpt = time.time()
         except KeyboardInterrupt:
             log.info("interrupted at step %d", self.step)
+            interrupted = True
         finally:
             self.close()
         log.info("Training complete, saving chkpt %s", os.path.join(a.checkpoint_dir, "on_stop.ckpt"))
-        return self.save("on_stop.ckpt")
+        # after an interrupt the other ranks may be anywhere in a step: no collective, rank 0 writes its state
+        return self.save("on_stop.ckpt", check_ranks=not interrupted)
 
 
 def main(argv=None):
@@ -396,6 +449,8 @@ def main(argv=None):
     args = parser.parse_args(argv)
     params = model_params(parser, args)
     refuse_untrainable(params, args.train_guide, args.guide_batch_stats)     # before any data is read
+    world = parallel.world_size() if dist.is_initialized() else int(os.environ.get("WORLD_SIZE", "1"))
+    data_pipeline.check_shard((0, world), args.batch_size)
     prefix = checkpoint.latest_checkpoint(args.checkpoint_dir)
     if prefix is not None:
         refuse_resume_mismatch(checkpoint.read_tf_checkpoint(prefix), args.train_guide)
@@ -403,7 +458,16 @@ def main(argv=None):
         log.warning("--profiling is accepted for compatibility and ignored")
     if not torch.cuda.is_available():
         raise RuntimeError("training needs a CUDA device; hdrnet_b200 has no CPU path")
-    return Trainer(args, params).run()
+    joined = False
+    if world > 1:
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")) % torch.cuda.device_count())
+        joined = not dist.is_initialized()
+        parallel.init_distributed()
+    try:
+        return Trainer(args, params).run()
+    finally:
+        if joined:
+            parallel.finalize()
 
 
 if __name__ == "__main__":

@@ -146,15 +146,21 @@ class Sampler:
     permutation of the n pairs (the identity without ``shuffle``).  Its flips (p = 1/2 each), its
     rotation k (uniform in 0..3) and its crop origin (uniform over the rotated extent, else the
     centre crop ``int((H - oh) / 2)``) come from a PCG64 stream seeded with ``(seed, step)``; the
-    draws are made whatever the flags, so enabling one augmentation does not move the others."""
+    draws are made whatever the flags, so enabling one augmentation does not move the others.
+
+    ``shard=(rank, world)`` names the part of each batch one rank of a data-parallel run builds:
+    rows ``[rank * B / world, (rank + 1) * B / world)`` of ``draws(step)`` (``shard_draws``);
+    ``batch_size`` stays the whole batch's, which ``world`` must divide."""
 
     def __init__(self, sizes, batch_size, output_resolution, shuffle=False, fliplr=False, flipud=False,
-                 rotate=False, random_crop=False, seed=0):
+                 rotate=False, random_crop=False, seed=0, shard=(0, 1)):
         self.sizes = [tuple(int(v) for v in s) for s in sizes]
         self.batch_size = int(batch_size)
         self.oh, self.ow = (int(v) for v in output_resolution)
         self.shuffle, self.fliplr, self.flipud = bool(shuffle), bool(fliplr), bool(flipud)
         self.rotate, self.random_crop, self.seed = bool(rotate), bool(random_crop), int(seed)
+        self.rank, self.world = check_shard(shard, self.batch_size)
+        self.shard_size = self.batch_size // self.world
         if not self.sizes:
             raise ValueError("no samples")
 
@@ -184,6 +190,23 @@ class Sampler:
                 cy, cx = int((rh - self.oh) / 2), int((rw - self.ow) / 2)     # tf.to_int32: truncation
             out.append(Draw(index, lr, ud, k, cy, cx))
         return out
+
+    def shard_draws(self, step: int) -> list:
+        """This shard's rows of ``draws(step)``."""
+        lo = self.rank * self.shard_size
+        return self.draws(step)[lo:lo + self.shard_size]
+
+
+def check_shard(shard, batch_size: int):
+    """``(rank, world)`` of ``shard``; ValueError unless 0 <= rank < world and world divides
+    ``batch_size`` (every rank builds an equal part of the batch)."""
+    rank, world = (int(v) for v in shard)
+    if world < 1 or not 0 <= rank < world:
+        raise ValueError(f"shard {tuple(shard)}: expected (rank, world) with 0 <= rank < world")
+    if int(batch_size) % world:
+        raise ValueError(f"the batch size {batch_size} is not a multiple of the world size {world}: every rank "
+                         "must build an equal part of the batch")
+    return rank, world
 
 
 def source_window(H: int, W: int, draw: Draw, oh: int, ow: int):
@@ -340,7 +363,7 @@ class HostStream:
         self.inputs, self.targets, self.sampler = inputs, targets, sampler
         self.oh, self.ow = (int(v) for v in output_resolution)
         self.device = device
-        self.slot_bytes = slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)}, sampler.batch_size,
+        self.slot_bytes = slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)}, sampler.shard_size,
                                      output_resolution)
         with torch.cuda.device(device):
             self.copy_stream = torch.cuda.Stream(device)
@@ -366,9 +389,9 @@ class HostStream:
 
     # ---- producer ------------------------------------------------------------------------------
     def _pack(self, slot: int, step: int) -> _Staged:
-        """Copy batch ``step``'s windows into pinned slot ``slot`` and upload it to device slot
-        ``slot`` on the copy stream."""
-        draws = self.sampler.draws(step)
+        """Copy batch ``step``'s windows (the sampler's shard of them) into pinned slot ``slot`` and
+        upload it to device slot ``slot`` on the copy stream."""
+        draws = self.sampler.shard_draws(step)
         layout, off = [], 0
         for d in draws:
             a, b = self.inputs[d.index], self.targets[d.index]
@@ -491,11 +514,17 @@ class ImageFilesDataPipeline:
     ``batch(step)`` returns the reference's sample dict for training step ``step``: ``image_input``,
     ``image_output`` [B, oh, ow, 3] and ``lowres_input`` [B, S, S, 3], float32 on ``device``, with
     S = ``params['net_input_size']`` (256 without params).  ``tier`` is ``"device"`` or ``"stream"``
-    (module docstring); ``close()`` (or leaving a ``with`` block) stops the streamed tier's threads."""
+    (module docstring); ``close()`` (or leaving a ``with`` block) stops the streamed tier's threads.
+
+    ``shard=(rank, world)``: one rank of a data-parallel run.  ``batch_size`` is the whole batch, and
+    ``batch(step)`` holds only this rank's B / world rows of it (``Sampler.shard_draws``), on either
+    tier; the streamed tier packs and uploads only their windows.  ValueError, before any file is
+    read, when ``world`` does not divide ``batch_size``."""
 
     def __init__(self, path, batch_size=32, output_resolution=(1080, 1920), shuffle=False, fliplr=False,
                  flipud=False, rotate=False, random_crop=False, params=None, nthreads=1, seed=0, device=None,
-                 memory_margin=MEMORY_MARGIN):
+                 memory_margin=MEMORY_MARGIN, shard=(0, 1)):
+        check_shard(shard, batch_size)
         self.path = path
         self.batch_size = int(batch_size)
         self.output_resolution = [int(v) for v in output_resolution]
@@ -505,12 +534,12 @@ class ImageFilesDataPipeline:
         self.names = names
         self.nsamples = len(names)
         self.sampler = Sampler([a.shape[:2] for a in inputs], batch_size, self.output_resolution, shuffle,
-                               fliplr, flipud, rotate, random_crop, seed)
+                               fliplr, flipud, rotate, random_crop, seed, shard)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         images = [im for pair in zip(inputs, targets) for im in pair]
         self.dataset_bytes = cache_bytes(images)
         self.staging_bytes = STREAM_SLOTS * slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)},
-                                                       self.batch_size, self.output_resolution)
+                                                       self.sampler.shard_size, self.output_resolution)
         self.tier = choose_tier(self.dataset_bytes, self.staging_bytes, self.device, memory_margin)
         self.stream = None
         if self.tier == "device":
@@ -528,7 +557,7 @@ class ImageFilesDataPipeline:
 
     def batch(self, step: int) -> dict:
         if self.stream is None:
-            draws = self.sampler.draws(step)
+            draws = self.sampler.shard_draws(step)
             fin, fout, low = train_batch([self.inputs[d.index] for d in draws],
                                          [self.targets[d.index] for d in draws],
                                          draws, self.output_resolution, self.net_input_size)

@@ -32,7 +32,9 @@ reference's training graph, with conv1 normalised by the batch's statistics
 (``csrc/guide_nn_grad.cu``), its moving averages updated in place on every call, and, with
 ``params['guide_grad']``, gradients for the guide's variables and ``fullres_input`` through
 ``_NNGuideFn``.  In the inference form (``is_training=False``) that guide is not differentiated.
-Batch-norm layers of the coefficient network and the pyramid model's resize are not differentiated:
+Under a process group of several ranks (data-parallel training, each rank holding a shard of the
+batch) the training-mode statistics are those of the whole batch: the ranks' input moments are
+merged before the fold (``parallel.moments_over_ranks``).  Batch-norm layers of the coefficient network and the pyramid model's resize are not differentiated:
 asking for their gradient raises ``NotImplementedError``.
 
 Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
@@ -50,7 +52,7 @@ import math
 import numpy as np
 import torch
 
-from . import _lib, layers
+from . import _lib, layers, parallel
 from .hdrnet_ops import _slice_apply_workspace, _workspace
 from .layers import bilateral_slice_apply
 
@@ -718,15 +720,18 @@ def _guide_grad(wts, params, x, names) -> bool:
                                  any(_requires_grad(wts.get("inference/guide/" + n)) for n in names))
 
 
-class _BatchStats(collections.namedtuple("_BatchStats", "npix moments guide mean var host")):
-    """conv1's batch statistics of one training-mode call: the input's moments (float64 [9]), the
-    _NNGuide on the folded weights the guide kernel runs with, the features' batch mean and biased
-    variance (float64), and the host copies (_host_f32) of the four variables they were folded from."""
+class _BatchStats(collections.namedtuple("_BatchStats", "npix moments guide mean var host count")):
+    """conv1's batch statistics of one training-mode call: this call's pixel count, the input's
+    moments (float64 [9]), the _NNGuide on the folded weights the guide kernel runs with, the
+    features' batch mean and biased variance (float64), the host copies (_host_f32) of the four
+    variables they were folded from, and the pixel count the statistics cover (npix, or the whole
+    batch's under a process group)."""
 
 
 def _nn_batch_stats(x, host) -> _BatchStats:
     """hdrnet_guide_nn_stats_f32 over x [B,H,W,3] (contiguous), one device-to-host copy of the 9
-    moments, then hdrnet_guide_nn_batch_fold in float64 on the host."""
+    moments, under a process group of several ranks their merge with the other ranks' moments
+    (parallel.moments_over_ranks), then hdrnet_guide_nn_batch_fold in float64 on the host."""
     lib = _lib.load()
     npix = x.numel() // 3
     w1, beta = host[0], host[1]
@@ -736,19 +741,21 @@ def _nn_batch_stats(x, host) -> _BatchStats:
     rc = lib.hdrnet_guide_nn_stats_f32(x.data_ptr(), npix, moments.data_ptr(), ws.data_ptr(), ws.numel() * 4,
                                        _stream(x.device))
     _lib.check(rc, "guide_nn batch statistics")
-    mom = np.ascontiguousarray(moments.cpu().numpy())
+    mom, count = parallel.moments_over_ranks(moments.cpu().numpy(), npix)
+    mom = np.ascontiguousarray(mom, np.float64)
     w1f, b1f = np.empty(3 * feats, np.float32), np.empty(feats, np.float32)
     mean, var = np.empty(feats, np.float64), np.empty(feats, np.float64)
     rc = lib.hdrnet_guide_nn_batch_fold(_hp(w1), _hp(beta), _hp(mom), feats, _hp(w1f), _hp(b1f), _hp(mean), _hp(var))
     _lib.check(rc, "guide_nn batch-norm fold")
-    return _BatchStats(npix, mom, _NNGuide(w1f, b1f, host[2], host[3]), mean, var, host)
+    return _BatchStats(npix, mom, _NNGuide(w1f, b1f, host[2], host[3]), mean, var, host, count)
 
 
 def _update_moving_averages(moving, stats: _BatchStats) -> None:
     """moving_mean and moving_variance toward the batch's statistics, in place, as TF's
     assign_moving_average without zero-debias: v -= (1 - decay) (v - batch).  The variance fed to it
-    is Bessel-corrected, var N / (N - 1) (1 for N = 1), as TF's fused batch norm does (DESIGN.md §5)."""
-    n = stats.npix
+    is Bessel-corrected, var N / (N - 1) (1 for N = 1), as TF's fused batch norm does (DESIGN.md §5),
+    with N the pixel count of the whole batch the statistics cover."""
+    n = stats.count
     unbiased = stats.var * (n / (n - 1.0) if n > 1 else 1.0)
     with torch.no_grad():
         for v, batch in zip(moving, (stats.mean, unbiased)):
@@ -1074,7 +1081,10 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
     def _guide(cls, input_tensor, params, is_training=False):
         """models.py:199-210 -> [B, H, W].  Inference form: conv1's batch norm folded from the moving
         averages.  ``is_training=True``: normalised with the batch's statistics (_nn_batch_stats), the
-        moving averages updated in place, and differentiable (_NNGuideFn) when _guide_grad says so."""
+        moving averages updated in place, and differentiable (_NNGuideFn) when _guide_grad says so.
+        Under a process group of several ranks the statistics are the whole batch's, every rank's
+        shard included; the parameter gradients are then this rank's share of the whole batch's
+        (their sum over the ranks), and ``fullres_input`` requiring grad raises NotImplementedError."""
         if is_training:
             wts = _resolve_weights(params)
             moving = _moving_averages(wts)
@@ -1083,6 +1093,11 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
             if x.numel() == 0:
                 raise ValueError("fullres_input is empty: batch statistics need at least one pixel")
             variables = [wts["inference/guide/" + n] for n in _NN_GUIDE_VARS]
+            if parallel.world_size() > 1 and _requires_grad(x) and _guide_grad(wts, params, x, _NN_GUIDE_VARS):
+                # each pixel's dinput depends on sums over the whole batch, which the VJP has for its own rank only
+                raise NotImplementedError(
+                    "the gradient of fullres_input through batch statistics taken over several ranks is not "
+                    "implemented: the guide's variables are differentiated, fullres_input must not require grad")
             with torch.cuda.device(x.device):
                 x = x.contiguous()
                 stats = _nn_batch_stats(x, [_host_f32(v) for v in variables])

@@ -7,9 +7,15 @@ design is one process per GPU, images sharded over ranks, and exactly ONE collec
 broadcast of the flat coefficient-network weight buffer (~1.93 MB) at init over NCCL
 (NVLink / NVSwitch); "nccl" on GPUs, "gloo" in the CPU tests.  The reference itself has no
 distributed code at all (SURVEY.md section 2b).
+
+Data-parallel training (bin/train.py under torchrun) adds, per step, one all-reduce of the flat
+gradient buffer (all_reduce_mean_) and one of a few scalars (sum_over_ranks); the pointwise-NN guide's
+training-mode batch norm adds one all-gather of the input moments (moments_over_ranks); and each
+checkpoint one all-gather of a digest of the state (check_ranks_agree).
 """
 from __future__ import annotations
 
+import hashlib
 import os
 
 import numpy as np
@@ -17,7 +23,9 @@ import torch
 import torch.distributed as dist
 
 __all__ = ["init_distributed", "shard_batch", "shard_rows", "shard_plan", "slice_apply_sharded",
-           "broadcast_weights", "max_over_ranks", "finalize", "bind_to_gpu_numa", "gpu_cpu_affinity"]
+           "broadcast_weights", "max_over_ranks", "finalize", "bind_to_gpu_numa", "gpu_cpu_affinity",
+           "world_size", "all_reduce_mean_", "sum_over_ranks", "merge_moments", "moments_over_ranks",
+           "check_ranks_agree"]
 
 
 def gpu_cpu_affinity(device_index: int) -> list[int]:
@@ -160,6 +168,107 @@ def max_over_ranks(value: float, device=None) -> float:
     t = torch.tensor([value], dtype=torch.float64, device=device)
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return float(t.item())
+
+
+def world_size() -> int:
+    """Ranks of the default process group; 1 when there is none."""
+    return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+
+
+def _staged(t: torch.Tensor) -> torch.Tensor:
+    """The tensor a collective works on: ``t`` itself with NCCL, a host copy with gloo."""
+    return t if dist.get_backend() == "nccl" else t.detach().cpu()
+
+
+def all_reduce_mean_(tensors) -> None:
+    """Average ``tensors`` (float32, same shapes on every rank) over the ranks, in place, with ONE
+    all-reduce of a single flat float32 buffer: with NCCL on the device, with gloo staged through the
+    host.  Every rank is left with the same bits.  Data-parallel training calls it on the gradients
+    after ``backward``: each rank's loss is the mean over its equal shard, so their average is the
+    gradient of the mean loss over the whole batch."""
+    world = world_size()
+    if world == 1 or not tensors:
+        return
+    flat = torch.cat([t.detach().reshape(-1) for t in tensors])
+    buf = _staged(flat)
+    dist.all_reduce(buf)
+    buf.div_(world)
+    if buf is not flat:
+        flat.copy_(buf)
+    off = 0
+    with torch.no_grad():
+        for t in tensors:
+            n = t.numel()
+            t.copy_(flat[off:off + n].view_as(t))
+            off += n
+
+
+def sum_over_ranks(values) -> np.ndarray:
+    """Sum a short float64 vector over the ranks (one all-reduce); ``values`` itself without a group."""
+    v = np.asarray(values, np.float64).reshape(-1)
+    if world_size() == 1:
+        return v
+    device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else "cpu"
+    t = torch.from_numpy(v.copy()).to(device)
+    dist.all_reduce(t)
+    return t.cpu().numpy()
+
+
+def _all_gather(t: torch.Tensor) -> np.ndarray:
+    """[world, *t.shape]: every rank's ``t``, in rank order, as a host array."""
+    buf = _staged(t.contiguous())
+    parts = [torch.empty_like(buf) for _ in range(world_size())]
+    dist.all_gather(parts, buf)
+    return torch.stack(parts).cpu().numpy()
+
+
+def merge_moments(counts, moments) -> np.ndarray:
+    """The moments of the union of disjoint pixel sets, in float64: ``counts[r]`` pixels with
+    ``moments[r]`` = (the mean of the 3 channels, then their biased covariance c00 c01 c02 c11 c12
+    c22), as hdrnet_guide_nn_stats_f32 computes them.  Each set's covariance is taken about the
+    union's mean, so a small variance about a large mean keeps its digits."""
+    n = np.asarray(counts, np.float64)
+    mom = np.asarray(moments, np.float64).reshape(len(n), 9)
+    total = n.sum()
+    if total == 0:
+        return np.zeros(9)
+    mean = (n[:, None] * mom[:, :3]).sum(0) / total
+    d = mom[:, :3] - mean
+    iu = np.triu_indices(3)
+    cov = (n[:, None] * (mom[:, 3:] + (d[:, :, None] * d[:, None, :])[:, iu[0], iu[1]])).sum(0) / total
+    return np.concatenate([mean, cov])
+
+
+def moments_over_ranks(moments, npix: int):
+    """(moments, pixels) of the whole batch from this rank's ``moments`` over its ``npix`` pixels:
+    one all-gather of every rank's (count, moments), merged by ``merge_moments`` in rank order, so
+    every rank gets the same bits.  Without a group: ``(moments, npix)`` unchanged."""
+    if world_size() == 1:
+        return np.asarray(moments, np.float64), int(npix)
+    row = torch.from_numpy(np.concatenate([[float(npix)], np.asarray(moments, np.float64).reshape(9)]))
+    if dist.get_backend() == "nccl":
+        row = row.to(torch.device("cuda", torch.cuda.current_device()))
+    rows = _all_gather(row)
+    return merge_moments(rows[:, 0], rows[:, 1:]), int(rows[:, 0].sum())
+
+
+def check_ranks_agree(arrays, what: str = "the training state") -> None:
+    """RuntimeError unless every rank holds the same bytes in ``arrays`` (host arrays, same order on
+    every rank): one all-gather of a 64-bit digest of them.  Nothing to do without a group."""
+    if world_size() == 1:
+        return
+    h = hashlib.blake2b(digest_size=8)
+    for a in arrays:
+        h.update(np.ascontiguousarray(a).tobytes())
+    mine = np.frombuffer(h.digest(), np.int64).copy()
+    t = torch.from_numpy(mine)
+    if dist.get_backend() == "nccl":
+        t = t.to(torch.device("cuda", torch.cuda.current_device()))
+    digests = _all_gather(t).reshape(-1)
+    if not (digests == digests[0]).all():
+        bad = [r for r in range(len(digests)) if digests[r] != digests[0]]
+        raise RuntimeError(f"{what} differs between ranks: ranks {bad} disagree with rank 0 (digests "
+                           f"{[hex(int(d) & (2 ** 64 - 1)) for d in digests]})")
 
 
 def finalize():

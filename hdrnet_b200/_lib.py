@@ -84,6 +84,8 @@ SIGNATURES = {
     "hdrnet_fuse_predict_grad_workspace_bytes": (ctypes.c_size_t, [_c_int] * 7),
     "hdrnet_fuse_predict_grad_f32": (_c_int, [_vp] * 8 + [_c_int] * 7 + [_vp, ctypes.c_size_t, _vp]),
     "hdrnet_resize_bilinear_f32":(_c_int, [_vp] * 3 + [_c_int] * 6 + [_vp]),
+    # (dout, din, B, H, W, C, OH, OW, stream)
+    "hdrnet_resize_bilinear_grad_f32": (_c_int, [_vp] * 2 + [_c_int] * 6 + [_vp]),
     "hdrnet_coefficients_scratch_bytes": (ctypes.c_size_t, [_c_int] * 7),
     "hdrnet_coefficients_f32": (_c_int, [_vp] * 4 + [_c_int, _vp, ctypes.c_size_t] + [_c_int] * 7 + [_vp]),
     # (samples, B, fullres_in, fullres_out, lowres_in, oh, ow, S, stream)

@@ -45,9 +45,21 @@ Adam slots, but go into every checkpoint and are restored on resume.  The flag i
 parameter and is not written to ``params.json``; a checkpoint does not record it, so a resume with the
 other setting is not refused: it only changes the guide's forward from then on.  ``--train_guide``
 with this model needs the flag; ``--guide_batch_stats`` with ``HDRNetCurves`` (no batch norm) is
-refused with ``ValueError``.  Training-mode batch norm in the coefficient network and the pyramid's
-resize VJP are not implemented, so ``--batch_norm``, ``HDRNetGaussianPyrNN`` and ``--train_guide``
-with ``HDRNetPointwiseNNGuide`` without ``--guide_batch_stats`` are refused before any data is read,
+refused with ``ValueError``.
+
+``HDRNetGaussianPyrNN`` has one pointwise-NN guide per pyramid level (``inference/guide/level_{0,1,2}``)
+and trains only as the reference's ``*_gpyrnn*.sh`` scripts train it: ``--nobatch_norm --train_guide
+--guide_batch_stats``.  Each step then runs ``inference(..., is_training=True)``: each level's conv1
+is normalised with that level's batch statistics, the three levels' moving averages move toward
+them, and the coefficient network and all three guides are trained in the same Adam, their
+gradients reaching the coarser levels through the VJP of the align-corners resize.  The three
+levels' moving averages get no Adam slots, go into every checkpoint and are restored on resume;
+evaluation and ``bin/run.py`` run the guide-fused inference form on them.  The pyramid without both
+flags would train through its inference form, which is not differentiated, so it is refused.
+
+Training-mode batch norm in the coefficient network is not implemented, so ``--batch_norm``, the
+pyramid without ``--train_guide --guide_batch_stats``, and ``--train_guide`` with
+``HDRNetPointwiseNNGuide`` without ``--guide_batch_stats`` are refused before any data is read,
 with the models' own ``NotImplementedError``.
 
 Data-parallel training on one host: ``torchrun --nproc-per-node N -m hdrnet_b200.bin.train ...``
@@ -129,11 +141,13 @@ def build_parser() -> argparse.ArgumentParser:
     train_grp.add_argument("--max_steps", type=int, default=None, help="stop when the global step reaches this (default: run until interrupted).")
     train_grp.add_argument("--seed", type=int, default=0, help="seed of the initial variables and of the data sampler.")
     train_grp.add_argument("--train_guide", dest="train_guide", action="store_true",
-                           help="train the curves guide's variables too, as the reference does (HDRNetCurves only).")
+                           help="train the guide's variables too, as the reference does (the pointwise-NN guide "
+                                "and the pyramid's guides need --guide_batch_stats).")
     train_grp.add_argument("--notrain_guide", dest="train_guide", action="store_false")
     train_grp.add_argument("--guide_batch_stats", dest="guide_batch_stats", action="store_true",
-                           help="run the pointwise-NN guide's batch norm in training mode (batch statistics, "
-                                "moving averages updated), as the reference does (HDRNetPointwiseNNGuide only).")
+                           help="run the pointwise-NN guides' batch norm in training mode (batch statistics, "
+                                "moving averages updated), as the reference does (HDRNetPointwiseNNGuide and "
+                                "HDRNetGaussianPyrNN).")
     train_grp.add_argument("--noguide_batch_stats", dest="guide_batch_stats", action="store_false")
 
     debug_grp = parser.add_argument_group("debug and profiling")
@@ -178,17 +192,26 @@ def model_params(parser, args) -> dict:
     return {a.dest: getattr(args, a.dest, None) for a in parser.model_group._group_actions}
 
 
+PYRAMID_FLAGS = "--train_guide --guide_batch_stats"
+
+
 def refuse_untrainable(params, train_guide=False, guide_batch_stats=False) -> None:
-    """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model,
-    training-mode batch norm in the coefficient network and (with ``train_guide``) the pointwise-NN
-    guide without ``guide_batch_stats``.  Asks the models themselves, on the CPU, with a stand-in
-    variable that requires grad (they refuse before any device work).  ValueError for
-    ``guide_batch_stats`` on ``HDRNetCurves``, whose guide has no batch norm."""
+    """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model
+    other than with ``train_guide`` and ``guide_batch_stats`` together, training-mode batch norm in
+    the coefficient network and (with ``train_guide``) the pointwise-NN guide without
+    ``guide_batch_stats``.  Asks the models themselves, on the CPU, with a stand-in variable that
+    requires grad (they refuse before any device work).  ValueError for ``guide_batch_stats`` on
+    ``HDRNetCurves``, whose guide has no batch norm."""
     S = int(params["net_input_size"])
-    if params["model_name"] == "HDRNetGaussianPyrNN":
+    if params["model_name"] == "HDRNetGaussianPyrNN" and not (train_guide and guide_batch_stats):
+        # the pyramid trains only as the reference's recipes train it: all three guides, in training mode
         probe = {COEFFS + "splat/conv1/weights": torch.zeros(1, requires_grad=True)}
-        models.HDRNetGaussianPyrNN.inference(torch.zeros(1, S, S, 3), torch.zeros(1, 1, 1, 3),
-                                             dict(params, weights=probe))
+        try:
+            models.HDRNetGaussianPyrNN.inference(torch.zeros(1, S, S, 3), torch.zeros(1, 1, 1, 3),
+                                                 dict(params, weights=probe))
+        except NotImplementedError as e:
+            raise NotImplementedError(f"{e}; {PYRAMID_FLAGS} trains the pyramid: its three guides, in "
+                                      "training mode") from None
     if params["batch_norm"]:
         probe = {f"{scope}/BatchNorm/beta": torch.zeros(1, requires_grad=True)
                  for scope, use_bn, _ in models._coefficient_specs(params) if use_bn}

@@ -2,12 +2,31 @@
 // Replaces tf.image.resize_images(..., BILINEAR, align_corners=True) as used by
 // HDRNetGaussianPyrNN._multiscale_input and ._output (hdrnet/models.py:249-289), TF1 legacy
 // semantics: src = dst * (in - 1) / (out - 1), lo = floor(src), hi = min(lo + 1, in - 1),
-// value = top + (bottom - top) * fy with top = tl + (tr - tl) * fx.
+// value = top + (bottom - top) * fy with top = tl + (tr - tl) * fx.  Its VJP
+// (hdrnet_resize_bilinear_grad_f32) gathers the transpose of that map; the fused add's VJP is the
+// identity and needs no kernel.
 #include <cuda_runtime.h>
 
 #include "hdrnet_b200.h"
 
 namespace hdrnet_b200 {
+
+// One output coordinate's source taps: src = o * s rounded to float32, lo = floor(src),
+// hi = min(lo + 1, n - 1), frac = src - lo.  The forward and its VJP both take their taps from
+// here, so the VJP sends each gradient back to exactly the pixels and weights the forward read.
+struct AcTaps {
+  int lo, hi;
+  float frac;
+};
+
+__device__ __forceinline__ AcTaps ac_taps(int o, float s, int n) {
+  // __fmul_rn: the product is rounded before frac = src - lo, in every caller.  A plain `o * s`
+  // may be contracted into fma(o, s, -lo) where the compiler rematerialises it, which gives a frac
+  // the forward never used.
+  const float src = __fmul_rn(static_cast<float>(o), s);
+  const int lo = static_cast<int>(floorf(src));
+  return {lo, min(lo + 1, n - 1), src - lo};
+}
 
 __global__ void __launch_bounds__(256)
 resize_bilinear_ac_kernel(const float* __restrict__ in, const float* __restrict__ add,
@@ -19,10 +38,9 @@ resize_bilinear_ac_kernel(const float* __restrict__ in, const float* __restrict_
     const int ox = static_cast<int>((e / C) % OW);
     const int oy = static_cast<int>((e / (static_cast<long long>(C) * OW)) % OH);
     const int b = static_cast<int>(e / (static_cast<long long>(C) * OW * OH));
-    const float fy_src = oy * sy, fx_src = ox * sx;
-    const int y0 = static_cast<int>(floorf(fy_src)), x0 = static_cast<int>(floorf(fx_src));
-    const int y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
-    const float fy = fy_src - y0, fx = fx_src - x0;
+    const AcTaps ty = ac_taps(oy, sy, H), tx = ac_taps(ox, sx, W);
+    const int y0 = ty.lo, y1 = ty.hi, x0 = tx.lo, x1 = tx.hi;
+    const float fy = ty.frac, fx = tx.frac;
     const float* img = in + static_cast<size_t>(b) * H * W * C;
     const float tl = __ldg(img + (static_cast<size_t>(y0) * W + x0) * C + c);
     const float tr = __ldg(img + (static_cast<size_t>(y0) * W + x1) * C + c);
@@ -33,6 +51,57 @@ resize_bilinear_ac_kernel(const float* __restrict__ in, const float* __restrict_
     float v = top + (bot - top) * fy;
     if (add) v += __ldg(add + e);
     out[e] = v;
+  }
+}
+
+// [first, last] output coordinates whose taps may reach input coordinate i: the inverse map of
+// src in [i - 1, i + 1), widened by one on each side for the rounding of src = o * s.  With s = 0
+// (n = 1, or one output) every output is a candidate.
+__device__ __forceinline__ int2 ac_candidates(int i, float s, int on) {
+  if (s == 0.0f) return make_int2(0, on - 1);
+  const float lo = floorf(static_cast<float>(i - 1) / s) - 1.0f;
+  const float hi = ceilf(static_cast<float>(i + 1) / s) + 1.0f;
+  return make_int2(static_cast<int>(fmaxf(lo, 0.0f)),
+                   static_cast<int>(fminf(hi, static_cast<float>(on - 1))));
+}
+
+// The weight output coordinate o's taps give input coordinate i, and whether they reach it at all:
+// (1 - frac) on lo, frac on hi, both where lo == hi on the last row or column.
+__device__ __forceinline__ bool ac_weight(int o, float s, int n, int i, float* w) {
+  const AcTaps t = ac_taps(o, s, n);
+  if (t.lo != i && t.hi != i) return false;
+  *w = (t.lo == i ? 1.0f - t.frac : 0.0f) + (t.hi == i ? t.frac : 0.0f);
+  return true;
+}
+
+// din[b, y, x, c] = sum over the output pixels whose taps reach (y, x) of wy * wx * dout, gathered
+// in a fixed order (output rows ascending, and within a row the columns ascending): no atomics, so
+// the result is the same bits on every run.
+__global__ void __launch_bounds__(256)
+resize_bilinear_ac_grad_kernel(const float* __restrict__ dout, float* __restrict__ din, int H,
+                               int W, int C, int OH, int OW, float sy, float sx,
+                               long long total) {
+  for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
+       e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(e % C);
+    const int x = static_cast<int>((e / C) % W);
+    const int y = static_cast<int>((e / (static_cast<long long>(C) * W)) % H);
+    const long long b = e / (static_cast<long long>(C) * W * H);
+    const int2 ry = ac_candidates(y, sy, OH), rx = ac_candidates(x, sx, OW);
+    const float* img = dout + b * OH * OW * C + c;
+    float acc = 0.0f;
+    for (int oy = ry.x; oy <= ry.y; ++oy) {
+      float wy;
+      if (!ac_weight(oy, sy, H, y, &wy)) continue;
+      const float* row = img + static_cast<long long>(oy) * OW * C;
+      float racc = 0.0f;
+      for (int ox = rx.x; ox <= rx.y; ++ox) {
+        float wx;
+        if (ac_weight(ox, sx, W, x, &wx)) racc = fmaf(wx, __ldg(row + static_cast<long long>(ox) * C), racc);
+      }
+      acc = fmaf(wy, racc, acc);
+    }
+    din[e] = acc;
   }
 }
 
@@ -51,6 +120,22 @@ extern "C" int hdrnet_resize_bilinear_f32(const float* in, const float* add, flo
   hdrnet_b200::resize_bilinear_ac_kernel<<<static_cast<unsigned>(blocks), 256, 0,
                                            static_cast<cudaStream_t>(stream)>>>(
       in, add, out, B, H, W, C, OH, OW, sy, sx, total);
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int hdrnet_resize_bilinear_grad_f32(const float* dout, float* din, int B, int H, int W,
+                                               int C, int OH, int OW, void* stream) {
+  if (B < 0 || H < 1 || W < 1 || C < 1 || OH < 1 || OW < 1) return HDRNET_E_BAD_SHAPE;
+  const long long total = static_cast<long long>(B) * H * W * C;
+  if (total == 0) return HDRNET_OK;
+  if (!dout || !din) return HDRNET_E_NULL_POINTER;
+  const float sy = (OH > 1) ? static_cast<float>(H - 1) / static_cast<float>(OH - 1) : 0.0f;
+  const float sx = (OW > 1) ? static_cast<float>(W - 1) / static_cast<float>(OW - 1) : 0.0f;
+  long long blocks = (total + 255) / 256;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
+  hdrnet_b200::resize_bilinear_ac_grad_kernel<<<static_cast<unsigned>(blocks), 256, 0,
+                                                static_cast<cudaStream_t>(stream)>>>(
+      dout, din, H, W, C, OH, OW, sy, sx, total);
   return static_cast<int>(cudaGetLastError());
 }
 

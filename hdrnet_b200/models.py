@@ -34,8 +34,13 @@ reference's training graph, with conv1 normalised by the batch's statistics
 ``_NNGuideFn``.  In the inference form (``is_training=False``) that guide is not differentiated.
 Under a process group of several ranks (data-parallel training, each rank holding a shard of the
 batch) the training-mode statistics are those of the whole batch: the ranks' input moments are
-merged before the fold (``parallel.moments_over_ranks``).  Batch-norm layers of the coefficient network and the pyramid model's resize are not differentiated:
-asking for their gradient raises ``NotImplementedError``.
+merged before the fold (``parallel.moments_over_ranks``).  ``HDRNetGaussianPyrNN`` has one such guide per
+pyramid level (``inference/guide/level_{0,1,2}``): ``inference(..., is_training=True)`` normalises each
+level with its own batch statistics and moves that level's moving averages, and differentiates the
+coefficient network and, with ``params['guide_grad']``, every level's guide and ``fullres_input``,
+through ``_ResizeFn``, whose backward is the VJP of the align-corners resize (``csrc/resize.cu``); its
+inference form is not differentiated.  Batch-norm layers of the coefficient network are not
+differentiated: asking for their gradient raises ``NotImplementedError``.
 
 Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
   coefficients  4 splat convs, 2 global convs + 3 FCs, 2 local convs (conv2d / fc kernels),
@@ -707,17 +712,18 @@ class _CurvesGuideFn(torch.autograd.Function):
         return (dx, *_split_param_grad(dp, ctx.needs_input_grad[1:], ctx.vars, _CURVES_GRAD_SLICES))
 
 
+GUIDE = "inference/guide"   # the guide's variable scope; the pyramid's levels are GUIDE/level_{l}
 _NN_GUIDE_VARS = ("conv1/weights", "conv1/BatchNorm/beta", "conv2/weights", "conv2/biases")
 _NN_MOVING = ("conv1/BatchNorm/moving_mean", "conv1/BatchNorm/moving_variance")
 
 
-def _guide_grad(wts, params, x, names) -> bool:
+def _guide_grad(wts, params, x, names, scope=GUIDE) -> bool:
     """Whether a guide goes through autograd: grad enabled, params['guide_grad'] truthy, and the input
-    or one of the guide's variables `names` (under inference/guide/) requiring grad."""
+    or one of the guide's variables `names` (under `scope`) requiring grad."""
     if not (torch.is_grad_enabled() and isinstance(params, dict) and params.get("guide_grad")):
         return False
     return _requires_grad(x) or (wts is not None and
-                                 any(_requires_grad(wts.get("inference/guide/" + n)) for n in names))
+                                 any(_requires_grad(wts.get(f"{scope}/{n}")) for n in names))
 
 
 class _BatchStats(collections.namedtuple("_BatchStats", "npix moments guide mean var host count")):
@@ -763,12 +769,12 @@ def _update_moving_averages(moving, stats: _BatchStats) -> None:
             v.sub_((v - b) * (1.0 - BN_DECAY))
 
 
-def _moving_averages(wts):
-    """The guide's moving averages, which training mode updates in place: float32 tensors that do not
-    require grad (TF does not train them)."""
+def _moving_averages(wts, scope=GUIDE):
+    """The moving averages of the NN guide under `scope`, which training mode updates in place:
+    float32 tensors that do not require grad (TF does not train them)."""
     out = []
     for n in _NN_MOVING:
-        key = "inference/guide/" + n
+        key = f"{scope}/{n}"
         v = wts.get(key) if isinstance(wts, dict) else None
         if not isinstance(v, torch.Tensor) or v.dtype != torch.float32:
             raise TypeError(f"{key} must be a float32 torch.Tensor: is_training=True updates it in place "
@@ -828,8 +834,8 @@ def _trainable_keys(wts, prefix: str):
 def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None, nn_guide=False,
                       is_training=False) -> None:
     """NotImplementedError for every gradient this package does not compute (checked before any
-    device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN).  The curves
-    guide's variables and fullres_input are differentiated only with params['guide_grad'], the
+    device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN's inference form).
+    The curves guide's variables and fullres_input are differentiated only with params['guide_grad'], the
     pointwise-NN guide's only with params['guide_grad'] and `is_training` (training-mode batch norm)."""
     if not torch.is_grad_enabled() or wts is None:
         return
@@ -837,8 +843,9 @@ def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=N
         wanted = _trainable_keys(wts, "inference/") + \
             [n for n, t in (("lowres_input", lowres_input), ("fullres_input", fullres_input)) if _requires_grad(t)]
         if wanted:
-            raise NotImplementedError(f"{what}: gradients are not implemented (requested for {wanted[0]}); "
-                                      "its _coefficients is differentiable on its own")
+            raise NotImplementedError(f"{what}: the inference form, with batch norm folded from the moving "
+                                      f"averages, is not differentiated (a gradient was requested for {wanted[0]}); "
+                                      "inference(..., is_training=True), the training graph, is")
         return
     guide = _trainable_keys(wts, "inference/guide")
     guide_grad = bool(params.get("guide_grad")) if isinstance(params, dict) else False
@@ -1078,22 +1085,23 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
         return cls._output(fullres_input, cls._guide(fullres_input, params, is_training=True), coeffs)
 
     @classmethod
-    def _guide(cls, input_tensor, params, is_training=False):
+    def _guide(cls, input_tensor, params, is_training=False, scope=GUIDE):
         """models.py:199-210 -> [B, H, W].  Inference form: conv1's batch norm folded from the moving
         averages.  ``is_training=True``: normalised with the batch's statistics (_nn_batch_stats), the
         moving averages updated in place, and differentiable (_NNGuideFn) when _guide_grad says so.
         Under a process group of several ranks the statistics are the whole batch's, every rank's
         shard included; the parameter gradients are then this rank's share of the whole batch's
-        (their sum over the ranks), and ``fullres_input`` requiring grad raises NotImplementedError."""
+        (their sum over the ranks), and ``fullres_input`` requiring grad raises NotImplementedError.
+        ``scope``: the training branch's variable scope (the pyramid's GUIDE/level_{l})."""
         if is_training:
             wts = _resolve_weights(params)
-            moving = _moving_averages(wts)
+            moving = _moving_averages(wts, scope)
             _refuse_untrained(wts, params, fullres_input=input_tensor, nn_guide=True, is_training=True)
             x = _check_input(input_tensor, "fullres_input")
             if x.numel() == 0:
                 raise ValueError("fullres_input is empty: batch statistics need at least one pixel")
-            variables = [wts["inference/guide/" + n] for n in _NN_GUIDE_VARS]
-            if parallel.world_size() > 1 and _requires_grad(x) and _guide_grad(wts, params, x, _NN_GUIDE_VARS):
+            variables = [wts[f"{scope}/{n}"] for n in _NN_GUIDE_VARS]
+            if parallel.world_size() > 1 and _requires_grad(x) and _guide_grad(wts, params, x, _NN_GUIDE_VARS, scope):
                 # each pixel's dinput depends on sums over the whole batch, which the VJP has for its own rank only
                 raise NotImplementedError(
                     "the gradient of fullres_input through batch statistics taken over several ranks is not "
@@ -1102,7 +1110,7 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
                 x = x.contiguous()
                 stats = _nn_batch_stats(x, [_host_f32(v) for v in variables])
                 _update_moving_averages(moving, stats)
-                if _guide_grad(wts, params, x, _NN_GUIDE_VARS):
+                if _guide_grad(wts, params, x, _NN_GUIDE_VARS, scope):
                     return _NNGuideFn.apply(x, *variables, stats)
                 return stats.guide.run(x)
         x = _check_input(input_tensor, "fullres_input")
@@ -1118,6 +1126,40 @@ def _resize(x: torch.Tensor, oh: int, ow: int, add: torch.Tensor | None = None) 
         torch.cuda.current_stream(x.device).cuda_stream)
     _lib.check(rc, "resize_bilinear")
     return out
+
+
+class _ResizeFn(torch.autograd.Function):
+    """_resize (+ fused add) over x and add: forward hdrnet_resize_bilinear_f32, the same kernel, so
+    the output keeps its bits; backward hdrnet_resize_bilinear_grad_f32 for x, and the identity for
+    add."""
+
+    @staticmethod
+    def forward(ctx, x, oh, ow, add=None):
+        x = x.contiguous()
+        ctx.in_hw = x.shape[1:3]
+        with torch.cuda.device(x.device):
+            return _resize(x, oh, ow, None if add is None else add.contiguous())
+
+    @staticmethod
+    def backward(ctx, dout):
+        dout = dout.contiguous()
+        din = None
+        if ctx.needs_input_grad[0]:
+            B, OH, OW, C = dout.shape
+            H, W = ctx.in_hw
+            din = torch.empty((B, H, W, C), dtype=torch.float32, device=dout.device)
+            with torch.cuda.device(dout.device):
+                rc = _lib.load().hdrnet_resize_bilinear_grad_f32(dout.data_ptr(), din.data_ptr(), B, H, W, C,
+                                                                 OH, OW, _stream(dout.device))
+            _lib.check(rc, "resize_bilinear VJP")
+        return din, None, None, (dout if ctx.needs_input_grad[3] else None)
+
+
+def _resize_maybe_grad(x, oh, ow, add=None):
+    """_resize, through _ResizeFn when grad is enabled and x or add requires it."""
+    if torch.is_grad_enabled() and (_requires_grad(x) or _requires_grad(add)):
+        return _ResizeFn.apply(x, oh, ow, add)
+    return _resize(x, oh, ow, add)
 
 
 class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
@@ -1144,8 +1186,16 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
 
     @classmethod
     def inference(cls, lowres_input, fullres_input, params, is_training=False):
+        """models.py:213-247.  The inference form (``is_training=False``) folds each level's conv1
+        batch norm from its moving averages and runs each level's guide inside its slice-apply; it
+        is not differentiated.  ``is_training=True`` is the reference's training graph
+        (hdrnet/bin/train.py:89-115), as HDRNetPointwiseNNGuide's: each level's guide normalises
+        conv1 with that level's batch statistics and moves ``level_{l}/conv1/BatchNorm/moving_mean``
+        and ``moving_variance`` toward them in place, once per call.  The coefficient variables and
+        ``lowres_input`` are differentiated; with ``params['guide_grad']`` so are each level's guide
+        variables and ``fullres_input``, through _NNGuideFn and the resize VJP (_ResizeFn)."""
         if is_training:
-            raise NotImplementedError("hdrnet_b200 implements the inference path only")
+            return cls._inference_training(lowres_input, fullres_input, params)
         _refuse_untrained(_weights_or_none(params), params, lowres_input, fullres_input,
                           what="HDRNetGaussianPyrNN.inference (needs the VJP of the align-corners resize)")
         fullres_input = _check_input(fullres_input, "fullres_input")
@@ -1160,6 +1210,30 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
         return out
 
     @classmethod
+    def _inference_training(cls, lowres_input, fullres_input, params):
+        """inference(..., is_training=True): every refusal on the CPU first, then the coefficients,
+        the pyramid, the three levels' guides (level 0 first, on every rank) and the coarse-to-fine
+        output through hdrnet_ops' slice-apply."""
+        wts = _resolve_weights(params)
+        if params.get("batch_norm"):
+            raise NotImplementedError(
+                "training-mode batch norm in the coefficient network (params['batch_norm']) is not "
+                "implemented: only the guides' conv1 batch norm runs in training mode")
+        for scope in cls._guide_scopes():
+            _moving_averages(wts, scope)
+        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True)
+        fullres_input = _check_input(fullres_input, "fullres_input")
+        coeffs = cls._coefficients(lowres_input, params)
+        with torch.cuda.device(fullres_input.device):
+            multiscale = cls._multiscale_input(fullres_input)
+            guides = cls._guide(multiscale, params, is_training=True)
+            return cls._output(multiscale, guides, coeffs, params)
+
+    @classmethod
+    def _guide_scopes(cls):
+        return [f"{GUIDE}/level_{il}" for il in range(cls.n_scales())]
+
+    @classmethod
     def inference_image(cls, image, params, lowres_image=None, out_dtype=torch.uint8):
         """Same contract as HDRNetCurves.inference_image.  The pyramid needs the float image at
         three scales, so only the network input is taken straight from the integer pixels; the
@@ -1172,24 +1246,31 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
 
     @classmethod
     def _multiscale_input(cls, fullres_input):
-        """models.py:249-262: each level is the previous one resized to floor(size / 2)."""
+        """models.py:249-262: each level is the previous one resized to floor(size / 2);
+        differentiable (_ResizeFn) when fullres_input requires grad."""
         lvls = [fullres_input]
         h, w = fullres_input.shape[1:3]
         for _ in range(cls.n_scales() - 1):
             h, w = h // 2, w // 2
-            lvls.append(_resize(lvls[-1], h, w))
+            lvls.append(_resize_maybe_grad(lvls[-1], h, w))
         return lvls
 
     @classmethod
     def _guide(cls, multiscale, params, is_training=False):
-        """models.py:264-272: HDRNetPointwiseNNGuide._guide per level (scope level_{il})."""
+        """models.py:264-272: HDRNetPointwiseNNGuide._guide per level (scope level_{il}).  In training
+        mode each level is normalised with its own batch statistics and updates its own moving
+        averages, the levels called in order."""
+        if is_training:
+            return [HDRNetPointwiseNNGuide._guide(lvl, params, True, scope)
+                    for lvl, scope in zip(multiscale, cls._guide_scopes())]
         prep = _prepare(_resolve_weights(params), params, multiscale[0].device, "pyramid")
         return [guide.run(lvl) for lvl, guide in zip(multiscale, prep.guides)]
 
     @classmethod
     def _output(cls, lvls, guide_lvls, coeffs, params=None):
         """models.py:274-289, coarse to fine.  With guide_lvls=None (the fast path) each level's
-        guide is computed inside its slice-apply kernel."""
+        guide is computed inside its slice-apply kernel; given the guides, hdrnet_ops' slice-apply
+        runs on them, and the upsample-and-add is differentiable (_ResizeFn) where grad is on."""
         prep = _prepare(_resolve_weights(params), params, lvls[0].device, "pyramid") \
             if guide_lvls is None else None
         B, gh, gw, gd = coeffs.shape[:4]
@@ -1203,7 +1284,7 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
                 out_lvl = bilateral_slice_apply(c, guide_lvls[src], lvl, has_offset=True)
             else:
                 out_lvl = _slice_apply_fused(c, lvl, prep.guides[src], torch.float32, False, False)[0]
-            current = out_lvl if il == 0 else _resize(current, H, W, add=out_lvl)
+            current = out_lvl if il == 0 else _resize_maybe_grad(current, H, W, add=out_lvl)
         return current
 
 

@@ -425,6 +425,16 @@ HDRNET_API int hdrnet_coefficients_f32(const float* lowres, float* grid, const f
 HDRNET_API int hdrnet_resize_bilinear_f32(const float* in, const float* add, float* out, int B,
                                           int H, int W, int C, int OH, int OW, void* stream);
 
+/*
+ * VJP of hdrnet_resize_bilinear_f32 (the fused add's VJP is the identity): din [B, H, W, C], the
+ * input-shaped gradient, from dout [B, OH, OW, C].  Each din element gathers the output pixels
+ * whose taps (the forward's own float32 lo / hi / frac) reach it, weighted (1-fy)(1-fx),
+ * (1-fy)fx, fy(1-fx) and fy fx, in a fixed order: no atomics, bitwise reproducible.  Every din
+ * element is written.  Same argument checks and return codes as the forward.
+ */
+HDRNET_API int hdrnet_resize_bilinear_grad_f32(const float* dout, float* din, int B, int H, int W,
+                                               int C, int OH, int OW, void* stream);
+
 /* The model-path forms with a lent workspace (B*H*gw*gd*48 bytes, as for
  * hdrnet_slice_apply_f32_ws): large images then run the texture-assisted kernel. */
 HDRNET_API int hdrnet_slice_apply_curves_f32_ws(const float* grid, const float* input, float* out,

@@ -3,7 +3,7 @@
 arguments and flags, hdrnet/bin/run.py:219-238):
 
     python -m hdrnet_b200.bin.run <checkpoint_dir> <input> <output> [--lowres_input X]
-                                  [--hdrp] [--debug] [--limit N]
+                                  [--hdrp] [--debug] [--limit N] [--output_bit_depth {8,16}]
 
 ``checkpoint_dir`` holds ``weights.npz`` (reference variable names, '/' written as '__') and
 ``params.json`` (the model_params the reference stores as graph constants, train.py:60-63,
@@ -15,6 +15,11 @@ Host-side pre/post processing follows the reference (run.py:139-190):
   (skimage.transform.resize(order=0), run.py:168-169) -> model -> uint8(255 * clip(out, 0, 1))
   (truncating cast, run.py:95) -> PNG.  Everything after the decode runs on the device, on the
   integer pixels (models.*.inference_image).
+
+``--output_bit_depth 16`` is an addition to the reference's CLI: the result is written as a 16-bit
+PNG, rint(65535 * clip(out, 0, 1)) from the same fused kernel, instead of the 8-bit cast that drops
+half the bits a model trained on 16-bit targets produces.  The default, 8, writes what the reference
+writes; the ``--debug`` pictures are 8-bit either way.
 """
 from __future__ import annotations
 
@@ -93,9 +98,10 @@ def save_checkpoint(checkpoint_dir, params, weights):
              **{k.replace("/", "__"): np.asarray(v) for k, v in weights.items()})
 
 
-def process(mdl, params, im_u: np.ndarray, lowres_u: np.ndarray | None = None, hdrp=False):
-    """One image through the model; returns uint8 HxWx3 (and the float output when
-    params['debug'] asks for the collections).
+def process(mdl, params, im_u: np.ndarray, lowres_u: np.ndarray | None = None, hdrp=False,
+            out_dtype=torch.uint8):
+    """One image through the model; returns uint8 HxWx3 -- uint16 with ``out_dtype=torch.uint16``
+    -- (and the float output when params['debug'] asks for the collections).
 
     The decoded uint8 / uint16 pixels go to the device as they are (3 or 6 bytes per pixel);
     img_as_float, the nearest-neighbour network input, the model and the uint8 cast all run
@@ -119,9 +125,9 @@ def process(mdl, params, im_u: np.ndarray, lowres_u: np.ndarray | None = None, h
         if lowres_u.ndim == 2:
             lowres_u = np.repeat(lowres_u[..., None], 3, axis=2)
         low_t = to_dev(lowres_u[:, :, :3])
-    out8 = mdl.inference_image(full_t, params, lowres_image=low_t)  # run.py:95 cast included
+    out_q = mdl.inference_image(full_t, params, lowres_image=low_t, out_dtype=out_dtype)  # run.py:95 cast included
     out = mdl.last_debug["output"] if params.get("debug") and hasattr(mdl, "last_debug") else None
-    return out8[0].cpu().numpy(), out
+    return out_q[0].cpu().numpy(), out
 
 
 def _to_png(x01: np.ndarray) -> np.ndarray:
@@ -152,6 +158,8 @@ def debug_images(im_rgb: np.ndarray, coeffs: np.ndarray, guides: list, multiscal
 
 def main(args):
     import cv2
+    # callers that build the namespace themselves may leave the flag out: 8, as the parser's default
+    out_dtype = OUTPUT_DTYPES[int(getattr(args, "output_bit_depth", 8))]
     params, _ = load_checkpoint(args.checkpoint_dir)
     mdl = getattr(models, params["model_name"])                     # run.py:82-85
     params["debug"] = bool(args.debug)
@@ -171,9 +179,9 @@ def main(args):
             lp = os.path.join(args.lowres_input, os.path.basename(path))
             lb = cv2.imread(lp, -1)
             low_u = lb[:, :, :3][:, :, ::-1] if lb is not None and lb.ndim == 3 else lb
-        out8, _ = process(mdl, params, np.ascontiguousarray(rgb), low_u, hdrp=args.hdrp)
+        out_q, _ = process(mdl, params, np.ascontiguousarray(rgb), low_u, hdrp=args.hdrp, out_dtype=out_dtype)
         name = os.path.splitext(os.path.basename(path))[0]
-        cv2.imwrite(os.path.join(args.output, name + ".png"), out8[:, :, ::-1])
+        cv2.imwrite(os.path.join(args.output, name + ".png"), out_q[:, :, ::-1])
         if args.debug:                                              # run.py:192-215
             dbg = mdl.last_debug
             guides = dbg["guide"] if isinstance(dbg["guide"], (list, tuple)) else [dbg["guide"]]
@@ -185,7 +193,11 @@ def main(args):
                 cv2.imwrite(os.path.join(args.output, name + fname), img)
 
 
-if __name__ == "__main__":
+# --output_bit_depth -> the dtype inference_image returns and cv2.imwrite stores
+OUTPUT_DTYPES = {8: torch.uint8, 16: torch.uint16}
+
+
+def build_parser() -> argparse.ArgumentParser:
     parser = argparse.ArgumentParser()
     parser.add_argument("checkpoint_dir", type=str, help="directory with weights.npz + params.json")
     parser.add_argument("input", type=str, help="image, directory of images, or filelist.txt")
@@ -195,5 +207,11 @@ if __name__ == "__main__":
     parser.add_argument("--nohdrp", dest="hdrp", action="store_false")
     parser.add_argument("--debug", dest="debug", action="store_true")
     parser.add_argument("--limit", type=int)
+    parser.add_argument("--output_bit_depth", type=int, choices=sorted(OUTPUT_DTYPES), default=8,
+                        help="8: uint8 PNGs, as the reference writes; 16: 16-bit PNGs, rint(65535 * clip)")
     parser.set_defaults(hdrp=False, debug=False)
-    main(parser.parse_args())
+    return parser
+
+
+if __name__ == "__main__":
+    main(build_parser().parse_args())

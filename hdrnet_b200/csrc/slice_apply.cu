@@ -376,6 +376,11 @@ slice_apply_px_generic_kernel(const float* __restrict__ grid, const unsigned cha
     if constexpr (kOut == kPxF32) {
       float* op = reinterpret_cast<float*>(out) + 3 * p;
       op[0] = o[0]; op[1] = o[1]; op[2] = o[2];
+    } else if constexpr (kOut == kPxU16) {
+      unsigned short* op = reinterpret_cast<unsigned short*>(out) + 3 * p;
+      op[0] = static_cast<unsigned short>(float_to_u16(o[0]));
+      op[1] = static_cast<unsigned short>(float_to_u16(o[1]));
+      op[2] = static_cast<unsigned short>(float_to_u16(o[2]));
     } else {
       out[3 * p] = static_cast<unsigned char>(float_to_u8(o[0]));
       out[3 * p + 1] = static_cast<unsigned char>(float_to_u8(o[1]));
@@ -883,6 +888,10 @@ static int launch_tma(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream, 
       return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU8, kPxU8>(a, fn, stream);
     if (in_fmt == kPxU16 && out_fmt == kPxU8)
       return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU16, kPxU8>(a, fn, stream);
+    if (in_fmt == kPxU8 && out_fmt == kPxU16)
+      return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU8, kPxU16>(a, fn, stream);
+    if (in_fmt == kPxU16 && out_fmt == kPxU16)
+      return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU16, kPxU16>(a, fn, stream);
   }
   if (in_fmt != kPxF32 || out_fmt != kPxF32) return HDRNET_E_UNSUPPORTED;
   return launch_tma_occ<GuideFn, kTexChunks, 2>(a, fn, stream);
@@ -982,6 +991,9 @@ static int launch_px_generic(const float* grid, const void* input, void* out, fl
   HDRNET_PX_CASE(kPxF32, kPxU8)
   HDRNET_PX_CASE(kPxU8, kPxF32)
   HDRNET_PX_CASE(kPxU16, kPxF32)
+  HDRNET_PX_CASE(kPxU8, kPxU16)
+  HDRNET_PX_CASE(kPxU16, kPxU16)
+  HDRNET_PX_CASE(kPxF32, kPxU16)
 #undef HDRNET_PX_CASE
   return HDRNET_E_UNSUPPORTED;
 }
@@ -1014,10 +1026,11 @@ static int plan_slice_apply(const SliceGeom& g, int n_in, int n_out, int has_off
   *f = ApplyForm{};
 
   // The persistent row kernels take the 3 -> 3 affine op with offset on 16-byte aligned, bulk-copy
-  // sized rows, with (u8 | u16) -> u8 or f32 -> f32 pixels; everything else runs a generic kernel.
+  // sized rows, with (u8 | u16) -> (u8 | u16) or f32 -> f32 pixels; everything else runs a generic
+  // kernel.
   TmaPlan plan;
   const bool row_shape = n_in == 3 && n_out == 3 && has_offset && aligned &&
-                         (!px || (in_fmt != kPxF32 && out_fmt == kPxU8)) &&
+                         (!px || (in_fmt != kPxF32 && (out_fmt == kPxU8 || out_fmt == kPxU16))) &&
                          make_tma_plan(g, max_smem, sms, &plan, false, kTmaThreads, in_fmt, out_fmt);
   // Texture-assisted forms: possible when the caller lent a workspace for the slab rows, at the
   // texture alignment.
@@ -1122,7 +1135,7 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
   const bool px = gs.in_fmt != kPxF32 || gs.out_fmt != kPxF32;
   if (px) {  // integer pixel I/O: model-path (fused-guide) forms of the 3 -> 3 affine op only
     if (gs.mode == 0 || n_in != 3 || n_out != 3 || !has_offset) return HDRNET_E_UNSUPPORTED;
-    if (gs.in_fmt < kPxF32 || gs.in_fmt > kPxU16 || (gs.out_fmt != kPxF32 && gs.out_fmt != kPxU8))
+    if (gs.in_fmt < kPxF32 || gs.in_fmt > kPxU16 || gs.out_fmt < kPxF32 || gs.out_fmt > kPxU16)
       return HDRNET_E_UNSUPPORTED;
   }
   int rc = validate_common(B, H, W, gh, gw, gd);
@@ -1131,6 +1144,17 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
   const long long npix = static_cast<long long>(B) * rows * W;
   if (npix == 0) return HDRNET_OK;
   if (!grid || !input || !out || (gs.mode == 0 && !gs.guide)) return HDRNET_E_NULL_POINTER;
+  if (gs.out_fmt == kPxU16) {
+    // A uint16 result has its own width (6 bytes per pixel against 3 / 6 / 12 in): written over its
+    // input or grid, a segment's store would overwrite pixels or coefficients other threads have not
+    // read yet.  These forms do not run in place.
+    const uintptr_t o0 = reinterpret_cast<uintptr_t>(out_v), o1 = o0 + static_cast<uintptr_t>(npix) * 6u;
+    const uintptr_t i0 = reinterpret_cast<uintptr_t>(input_v),
+                    i1 = i0 + static_cast<uintptr_t>(npix) * 3u * px_bytes_per_channel(gs.in_fmt);
+    const uintptr_t g0 = reinterpret_cast<uintptr_t>(grid),
+                    g1 = g0 + static_cast<uintptr_t>(B) * gh * gw * gd * kGc * sizeof(float);
+    if ((o0 < i1 && i0 < o1) || (o0 < g1 && g0 < o1)) return HDRNET_E_UNSUPPORTED;
+  }
   const int J = n_in + (has_offset ? 1 : 0);
   const long long grid_floats = static_cast<long long>(gh) * gw * gd * n_out * J;
   if (grid_floats > INT_MAX || static_cast<long long>(rows) * B > INT_MAX / 4) return HDRNET_E_TOO_LARGE;

@@ -576,6 +576,8 @@ int launch_async_fused(const TmaArgs& a, const CurvesGuideParams& curves, int in
   if (in_fmt == kPxF32 && out_fmt == kPxF32) return launch_async_fused_fmt<kPxF32, kPxF32>(a, fn, stream);
   if (in_fmt == kPxU8 && out_fmt == kPxU8) return launch_async_fused_fmt<kPxU8, kPxU8>(a, fn, stream);
   if (in_fmt == kPxU16 && out_fmt == kPxU8) return launch_async_fused_fmt<kPxU16, kPxU8>(a, fn, stream);
+  if (in_fmt == kPxU8 && out_fmt == kPxU16) return launch_async_fused_fmt<kPxU8, kPxU16>(a, fn, stream);
+  if (in_fmt == kPxU16 && out_fmt == kPxU16) return launch_async_fused_fmt<kPxU16, kPxU16>(a, fn, stream);
   return HDRNET_E_UNSUPPORTED;
 }
 

@@ -17,7 +17,8 @@ namespace hdrnet_b200 {
 // =========================================================================================
 // Pixel storage formats of the model-path forms (row f-3): the full-resolution image may stay
 // in the integer format it was decoded to, and the result may leave as the uint8 the reference
-// writes (hdrnet/bin/run.py:145-169 img_as_float; :95 uint8(255 * clip(out, 0, 1))).
+// writes (hdrnet/bin/run.py:145-169 img_as_float; :95 uint8(255 * clip(out, 0, 1))) or as uint16
+// (row f-11: the 16 bits the model is trained to produce).
 // =========================================================================================
 constexpr int kPxF32 = HDRNET_PX_F32, kPxU8 = HDRNET_PX_U8, kPxU16 = HDRNET_PX_U16;
 
@@ -40,6 +41,15 @@ __device__ __forceinline__ float px_to_float(unsigned v) {
 // tf.cast(255.0 * tf.clip_by_value(x, 0, 1), tf.uint8): truncating conversion.
 __device__ __forceinline__ unsigned float_to_u8(float x) {
   return __float2uint_rz(255.0f * fminf(fmaxf(x, 0.0f), 1.0f));
+}
+
+// The 16-bit result: rint(65535 * clip(x, 0, 1)), round to nearest even -- how the project writes
+// 16-bit targets (np.rint(np.clip(x, 0, 1) * 65535)).  Rounding, not the truncation of float_to_u8
+// (which follows tf.cast in run.py:95), so that an identity model returns every uint16 code value
+// unchanged: float32(v / 65535) * 65535 can land just below v, and truncation would give v - 1.
+// NaN maps to 0 (fmaxf returns the non-NaN operand), as in float_to_u8.
+__device__ __forceinline__ unsigned float_to_u16(float x) {
+  return __float2uint_rn(65535.0f * fminf(fmaxf(x, 0.0f), 1.0f));
 }
 
 // One thread's 4 consecutive pixels, from / to a staged tile (shared memory) or global memory.
@@ -81,12 +91,17 @@ __device__ __forceinline__ void store_quad(unsigned char* tile, int q, const flo
     rgb4[0] = make_float4(o_r[0], o_g[0], o_b[0], o_r[1]);
     rgb4[1] = make_float4(o_g[1], o_b[1], o_r[2], o_g[2]);
     rgb4[2] = make_float4(o_b[2], o_r[3], o_g[3], o_b[3]);
-  } else {
-    static_assert(kFmt == kPxU8, "results leave as float32 or uint8");
+  } else if constexpr (kFmt == kPxU8) {
     uint32_t* w = reinterpret_cast<uint32_t*>(tile) + 3 * q;
     w[0] = float_to_u8(o_r[0]) | (float_to_u8(o_g[0]) << 8) | (float_to_u8(o_b[0]) << 16) | (float_to_u8(o_r[1]) << 24);
     w[1] = float_to_u8(o_g[1]) | (float_to_u8(o_b[1]) << 8) | (float_to_u8(o_r[2]) << 16) | (float_to_u8(o_g[2]) << 24);
     w[2] = float_to_u8(o_b[2]) | (float_to_u8(o_r[3]) << 8) | (float_to_u8(o_g[3]) << 16) | (float_to_u8(o_b[3]) << 24);
+  } else {
+    static_assert(kFmt == kPxU16, "results leave as float32, uint8 or uint16");
+    uint2* w = reinterpret_cast<uint2*>(tile) + 3 * q;                  // 24 bytes
+    w[0] = make_uint2(float_to_u16(o_r[0]) | (float_to_u16(o_g[0]) << 16), float_to_u16(o_b[0]) | (float_to_u16(o_r[1]) << 16));
+    w[1] = make_uint2(float_to_u16(o_g[1]) | (float_to_u16(o_b[1]) << 16), float_to_u16(o_r[2]) | (float_to_u16(o_g[2]) << 16));
+    w[2] = make_uint2(float_to_u16(o_b[2]) | (float_to_u16(o_r[3]) << 16), float_to_u16(o_g[3]) | (float_to_u16(o_b[3]) << 16));
   }
 }
 

@@ -28,11 +28,14 @@ class HostImagePipeline:
 
     frames: [N, H, W, 3] uint8 / uint16 / float32 CPU tensor (pinned memory for asynchronous
     copies; pageable memory works but serialises).  Returns / fills ``out`` [N, H, W, 3] uint8 (or
-    float32 with ``out_dtype=torch.float32``) on the CPU.  ``frames_per_step`` frames travel and
+    uint16 / float32 with ``out_dtype=torch.uint16`` / ``torch.float32``) on the CPU, page-locked
+    when ``frames`` is.  ``frames_per_step`` frames travel and
     run together (1 = lowest latency per frame and the best overlap)."""
 
     def __init__(self, model_cls, params, device=None, depth: int = 2, frames_per_step: int = 1,
                  out_dtype=torch.uint8):
+        from .models import _check_out_dtype
+        _check_out_dtype(out_dtype)
         if not torch.cuda.is_available():
             raise _lib.HdrnetLibraryError("HostImagePipeline needs a CUDA device: hdrnet_b200 has no CPU path")
         self.model_cls, self.params, self.out_dtype = model_cls, params, out_dtype

@@ -454,6 +454,23 @@ def quantize_u8(x: torch.Tensor) -> torch.Tensor:
     return (255.0 * x.clamp(0.0, 1.0)).to(torch.uint8)
 
 
+def quantize_u16(x: torch.Tensor) -> torch.Tensor:
+    """rint(65535 * clip(x, 0, 1)) in float32, round half to even, NaN -> 0: the uint16 epilogue of
+    the fused slice-apply kernels (csrc/slice_rows.cuh float_to_u16), for results computed in float."""
+    y = torch.round(65535.0 * x.nan_to_num(nan=0.0).clamp(0.0, 1.0))
+    return y.to(torch.int32).to(torch.uint16)
+
+
+# What inference_image / inference_image_host return: the reference's uint8 cast, the 16-bit result
+# (rint(65535 * clip)), or the unquantised prediction.
+OUT_DTYPES = (torch.uint8, torch.uint16, torch.float32)
+
+
+def _check_out_dtype(out_dtype) -> None:
+    if out_dtype not in OUT_DTYPES:
+        raise TypeError(f"out_dtype must be torch.uint8, torch.uint16 or torch.float32, got {out_dtype}")
+
+
 def pack_conv_weights(w: torch.Tensor):
     """Pre-pack HWIO conv weights for the pipelined tensor-core (wgmma) kernel (once per model); returns a
     device buffer, or None when the layer's shape does not suit that kernel."""
@@ -927,7 +944,10 @@ class HDRNetCurves(object):
         -> coefficients -> guide + slice + apply in one full-resolution pass that reads the
         integer pixels and writes ``uint8(255 * clip(out, 0, 1))`` (run.py:95).  3 + 3 bytes per
         pixel cross PCIe / HBM instead of 12 + 12.  ``lowres_image`` replaces the resized input
-        (run.py --lowres_input); ``out_dtype=torch.float32`` returns the unquantised prediction."""
+        (run.py --lowres_input); ``out_dtype=torch.float32`` returns the unquantised prediction and
+        ``out_dtype=torch.uint16`` the 16-bit one, ``rint(65535 * clip(out, 0, 1))`` written by the
+        same kernel (6 bytes per pixel).  Any other ``out_dtype`` is a TypeError."""
+        _check_out_dtype(out_dtype)
         image = _check_image(image, "image")
         src = image if lowres_image is None else _check_image(lowres_image, "lowres_image")
         lowres = lowres_from_image(src, int(params["net_input_size"]))
@@ -939,8 +959,10 @@ class HDRNetCurves(object):
         """``inference_image`` for frames that live in HOST memory (what hdrnet/bin/run.py does per
         file: load, ``sess.run``, save): uploads, the model and downloads of consecutive frames
         overlap on three streams (hdrnet_b200/host_pipeline.py).  ``frames`` [N,H,W,3] uint8 /
-        uint16 / float32 CPU tensor (pinned for asynchronous copies) -> CPU tensor of ``out_dtype``.
-        One pipeline (streams + two frame buffers) is kept per (class, device, out_dtype)."""
+        uint16 / float32 CPU tensor (pinned for asynchronous copies) -> CPU tensor of ``out_dtype``
+        (uint8, uint16 or float32).  One pipeline (streams + two frame buffers) is kept per (class,
+        device, out_dtype)."""
+        _check_out_dtype(out_dtype)
         from .host_pipeline import HostImagePipeline
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         key = (cls, dev, out_dtype)
@@ -1237,12 +1259,16 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
     def inference_image(cls, image, params, lowres_image=None, out_dtype=torch.uint8):
         """Same contract as HDRNetCurves.inference_image.  The pyramid needs the float image at
         three scales, so only the network input is taken straight from the integer pixels; the
-        full-resolution image is converted once on the device."""
+        full-resolution image is converted once on the device.  The float result of the three
+        levels' sum is quantised once, on the device (quantize_u8 / quantize_u16)."""
+        _check_out_dtype(out_dtype)
         image = _check_image(image, "image")
         src = image if lowres_image is None else _check_image(lowres_image, "lowres_image")
         lowres = lowres_from_image(src, int(params["net_input_size"]))
         out = cls.inference(lowres, image_to_float(image), params, False)
-        return quantize_u8(out) if out_dtype == torch.uint8 else out
+        if out_dtype == torch.uint8:
+            return quantize_u8(out)
+        return quantize_u16(out) if out_dtype == torch.uint16 else out
 
     @classmethod
     def _multiscale_input(cls, fullres_input):

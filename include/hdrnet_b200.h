@@ -460,15 +460,18 @@ HDRNET_API int hdrnet_slice_apply_nn_f32_ws(const float* grid, const float* inpu
  */
 #define HDRNET_PX_F32 0 /* float32 [B,H,W,3]                                              */
 #define HDRNET_PX_U8 1  /* uint8   [B,H,W,3]; as input: img_as_float; as output: the cast  */
-#define HDRNET_PX_U16 2 /* uint16  [B,H,W,3]; input only                                  */
+#define HDRNET_PX_U16 2 /* uint16  [B,H,W,3]; as input: img_as_float; as output: rint(65535 * clip) */
 
 /*
  * hdrnet_slice_apply_{curves,nn}_f32_ws with `input` in in_fmt and `out` in out_fmt
- * (HDRNET_PX_F32 or HDRNET_PX_U8).  The conversion of a code value is bit-exact with
- * float32(float64(v) / 255) (resp. 65535); the uint8 cast truncates like tf.cast.  (u8 | u16) ->
- * u8 with W % 16 == 0 (W % 8 for u16) and 16-byte aligned buffers runs the persistent row kernel;
- * every other combination runs a one-thread-per-pixel fused kernel.  guide_out (optional)
- * receives the float32 guide map.  f32 -> f32 is hdrnet_slice_apply_{curves,nn}_f32_ws itself.
+ * (HDRNET_PX_F32, HDRNET_PX_U8 or HDRNET_PX_U16).  The conversion of a code value is bit-exact with
+ * float32(float64(v) / 255) (resp. 65535); the uint8 cast truncates like tf.cast; the uint16 result
+ * is rint(65535 * clip(x, 0, 1)), rounded to nearest even, so an identity model returns every
+ * uint16 code unchanged; NaN gives 0 in both.  (u8 | u16) -> (u8 | u16) with W % 16 == 0 (W % 8
+ * when both sides are u16) and 16-byte aligned buffers runs the persistent row kernel; every other
+ * combination runs a one-thread-per-pixel fused kernel.  A uint16 `out` must not overlap `input`
+ * or `grid` (HDRNET_E_UNSUPPORTED).  guide_out (optional) receives the float32 guide map.
+ * f32 -> f32 is hdrnet_slice_apply_{curves,nn}_f32_ws itself.
  */
 HDRNET_API int hdrnet_slice_apply_curves_px_ws(const float* grid, const void* input, int in_fmt,
                                                void* out, int out_fmt, float* guide_out, int B,

@@ -18,8 +18,8 @@ HEADER_PATH = os.path.normpath(os.path.join(_HERE, "..", "include", "hdrnet_b200
 
 # Return codes (include/hdrnet_b200.h)
 OK = 0
-E_NULL_POINTER, E_BAD_SHAPE, E_BAD_CHANNELS, E_TOO_LARGE, E_UNSUPPORTED, E_BAD_CONTEXT = (
-    -1, -2, -3, -4, -5, -6)
+E_NULL_POINTER, E_BAD_SHAPE, E_BAD_CHANNELS, E_TOO_LARGE, E_UNSUPPORTED, E_BAD_CONTEXT, E_BAD_MODEL = (
+    -1, -2, -3, -4, -5, -6, -7)
 VARIANT_AUTO, VARIANT_GENERIC, VARIANT_TMA, VARIANT_TEX, VARIANT_TEX_ASYNC = 0, 1, 2, 4, 7
 
 _c_int = ctypes.c_int
@@ -93,6 +93,14 @@ SIGNATURES = {
     "hdrnet_host_ctx_create": (_c_int, [ctypes.POINTER(_vp), ctypes.c_size_t]),
     "hdrnet_host_ctx_destroy": (_c_int, [_vp]),
     "hdrnet_slice_apply_host_f32": (_c_int, [_vp] * 5 + [_c_int] * 9),
+    # the whole-model object (frozen model file -> hdrnet_model*)
+    "hdrnet_model_create": (_c_int, [ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(_vp)]),
+    "hdrnet_model_destroy": (_c_int, [_vp]),
+    "hdrnet_model_info": (_c_int, [_vp] + [ctypes.POINTER(_c_int)] * 6),
+    "hdrnet_model_workspace_bytes": (ctypes.c_size_t, [_vp] + [_c_int] * 5),
+    # (model, image, in_fmt, lowres, lowres_fmt, SH, SW, out, out_fmt, B, H, W, ws, bytes, stream)
+    "hdrnet_model_run_px": (_c_int, [_vp, _vp, _c_int, _vp] + [_c_int] * 3 + [_vp] + [_c_int] * 4
+                            + [_vp, ctypes.c_size_t, _vp]),
 }
 
 # pixel storage formats (include/hdrnet_b200.h HDRNET_PX_*)

@@ -634,3 +634,101 @@ def import_checkpoint(checkpoint_dir: str, verify: bool = False, legacy: bool = 
     weights = upgrade_legacy_names(variables) if legacy else model_weights(variables)
     params = read_meta_model_params(prefix + ".meta") if os.path.exists(prefix + ".meta") else None
     return params, weights
+
+
+# ---------------------------------------------------------------------------------------------
+# Frozen model file: the arrays the kernels consume, for the whole-model C-ABI (hdrnet_model_create)
+# ---------------------------------------------------------------------------------------------
+# Layout (little-endian; csrc/model.cu and DESIGN.md row f-12 describe the same bytes):
+#   char[8] magic | u32 version | u32 kind | i32 net_input_size, spatial_bin, luma_bins,
+#   channel_multiplier, guide width | u32 array count | per array: u32 ndim, u32 dims[ndim],
+#   float32 data | u32 CRC-32C of every byte before it.
+FROZEN_MAGIC = b"HDRNETFZ"
+FROZEN_VERSION = 1
+FROZEN_KINDS = ("HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN")   # kind = index
+_FROZEN_HEADER = struct.Struct("<8sII5iI")
+
+
+def frozen_arrays(weights: dict, params: dict) -> list:
+    """The arrays of the frozen file, in its order, as float32 numpy: each coefficient-network layer's
+    weights and bias (an empty array for a layer without one) as ``models._Prepared`` builds them --
+    batch norm folded by ``models._fold`` -- then the guide: the curves guide's ccm, ccm_bias, shifts,
+    slopes, mix and [mix_bias], or the folded w1, b1, w2 and [b2] of each pointwise-NN guide (one per
+    pyramid level)."""
+    import torch
+
+    from . import models
+    name = params.get("model_name", "HDRNetCurves")
+    if name not in FROZEN_KINDS:
+        raise ValueError(f"model_name {name!r} is not one of {FROZEN_KINDS}")
+    prep = models._Prepared(weights, params, torch.device("cpu"), getattr(models, name)._nn_guide)
+    out = []
+    for scope, _, _ in models._coefficient_specs(params):
+        w, b, _ = prep.layers[scope]
+        out.append(w.detach().numpy())
+        out.append(np.zeros(0, np.float32) if b is None else b.detach().numpy())
+    for g in prep.guides:
+        if isinstance(g, models._CurvesGuide):
+            out += [g.ccm, g.ccm_bias, g.shifts, g.slopes, g.mix, np.array([g.mix_bias], np.float32)]
+        else:
+            out += [g.w1, g.b1, g.w2, np.array([g.b2], np.float32)]
+    return [np.ascontiguousarray(a, np.float32) for a in out]
+
+
+def _frozen_bytes(kind: int, hyper, arrays) -> bytes:
+    parts = [_FROZEN_HEADER.pack(FROZEN_MAGIC, FROZEN_VERSION, kind, *hyper, len(arrays))]
+    for a in arrays:
+        parts.append(struct.pack(f"<I{a.ndim}I", a.ndim, *a.shape))
+        parts.append(np.ascontiguousarray(a, "<f4").tobytes())
+    body = b"".join(parts)
+    return body + struct.pack("<I", crc32c(body))
+
+
+def freeze_model(weights: dict, params: dict, path: str) -> str:
+    """Write the frozen model file of (weights, params) to `path`: what hdrnet_model_create (and
+    ``hdrnet_b200.frozen.FrozenModel``, and the ``hdrnet_run`` program) load.  Returns `path`."""
+    arrays = frozen_arrays(weights, params)
+    name = params.get("model_name", "HDRNetCurves")
+    width = 16 if name == "HDRNetCurves" else int(arrays[-4].shape[1])
+    hyper = (int(params["net_input_size"]), int(params["spatial_bin"]), int(params["luma_bins"]),
+             int(params["channel_multiplier"]), width)
+    data = _frozen_bytes(FROZEN_KINDS.index(name), hyper, arrays)
+    with open(path, "wb") as f:
+        f.write(data)
+    return path
+
+
+def read_frozen_model(path: str) -> dict:
+    """A frozen model file back: ``model_name``, ``net_input_size``, ``spatial_bin``, ``luma_bins``,
+    ``channel_multiplier``, ``guide_width`` and ``arrays`` (the list frozen_arrays gave).  Raises
+    ValueError for a wrong magic, version, length or CRC-32C (shapes are the C side's to check)."""
+    with open(path, "rb") as f:
+        data = f.read()
+    if len(data) < _FROZEN_HEADER.size + 4 or data[:8] != FROZEN_MAGIC:
+        raise ValueError(f"{path}: not a frozen hdrnet_b200 model")
+    magic, version, kind, S, sb, gd, cm, width, n = _FROZEN_HEADER.unpack_from(data)
+    if version != FROZEN_VERSION:
+        raise ValueError(f"{path}: frozen model format version {version}, this reader knows {FROZEN_VERSION}")
+    if crc32c(data[:-4]) != struct.unpack_from("<I", data, len(data) - 4)[0]:
+        raise ValueError(f"{path}: CRC-32C mismatch")
+    if kind >= len(FROZEN_KINDS):
+        raise ValueError(f"{path}: unknown model kind {kind}")
+    arrays, off = [], _FROZEN_HEADER.size
+    end = len(data) - 4
+    for _ in range(n):
+        if off + 4 > end:
+            raise ValueError(f"{path}: truncated array header")
+        (ndim,) = struct.unpack_from("<I", data, off)
+        if off + 4 + 4 * ndim > end:
+            raise ValueError(f"{path}: truncated array header")
+        shape = struct.unpack_from(f"<{ndim}I", data, off + 4)
+        off += 4 + 4 * ndim
+        count = int(np.prod(shape, dtype=np.int64))
+        if off + 4 * count > end:
+            raise ValueError(f"{path}: truncated array")
+        arrays.append(np.frombuffer(data, "<f4", count, off).reshape(shape).astype(np.float32))
+        off += 4 * count
+    if off != end:
+        raise ValueError(f"{path}: {end - off} bytes after the last array")
+    return dict(model_name=FROZEN_KINDS[kind], net_input_size=S, spatial_bin=sb, luma_bins=gd,
+                channel_multiplier=cm, guide_width=width, arrays=arrays)

@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include "hdrnet_b200.h"
+#include "slice_rows.cuh"
 
 namespace hdrnet_b200 {
 
@@ -28,29 +29,54 @@ __device__ __forceinline__ AcTaps ac_taps(int o, float s, int n) {
   return {lo, min(lo + 1, n - 1), src - lo};
 }
 
+// Output element e of the resize (+ add): the one arithmetic of the float forward and of its
+// quantising form below, so both compute the same float.
+__device__ __forceinline__ float resize_ac_value(const float* __restrict__ in, const float* __restrict__ add,
+                                                 int H, int W, int C, int OH, int OW, float sy,
+                                                 float sx, long long e) {
+  const int c = static_cast<int>(e % C);
+  const int ox = static_cast<int>((e / C) % OW);
+  const int oy = static_cast<int>((e / (static_cast<long long>(C) * OW)) % OH);
+  const int b = static_cast<int>(e / (static_cast<long long>(C) * OW * OH));
+  const AcTaps ty = ac_taps(oy, sy, H), tx = ac_taps(ox, sx, W);
+  const int y0 = ty.lo, y1 = ty.hi, x0 = tx.lo, x1 = tx.hi;
+  const float fy = ty.frac, fx = tx.frac;
+  const float* img = in + static_cast<size_t>(b) * H * W * C;
+  const float tl = __ldg(img + (static_cast<size_t>(y0) * W + x0) * C + c);
+  const float tr = __ldg(img + (static_cast<size_t>(y0) * W + x1) * C + c);
+  const float bl = __ldg(img + (static_cast<size_t>(y1) * W + x0) * C + c);
+  const float br = __ldg(img + (static_cast<size_t>(y1) * W + x1) * C + c);
+  const float top = tl + (tr - tl) * fx;
+  const float bot = bl + (br - bl) * fx;
+  float v = top + (bot - top) * fy;
+  if (add) v += __ldg(add + e);
+  return v;
+}
+
 __global__ void __launch_bounds__(256)
 resize_bilinear_ac_kernel(const float* __restrict__ in, const float* __restrict__ add,
                           float* __restrict__ out, int B, int H, int W, int C, int OH, int OW,
                           float sy, float sx, long long total) {
   for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
+       e += static_cast<long long>(gridDim.x) * blockDim.x)
+    out[e] = resize_ac_value(in, add, H, W, C, OH, OW, sy, sx, e);
+}
+
+// The same resize (+ add) with the model path's quantising epilogue: the uint8 cast of
+// tf.cast(255 * clip(v, 0, 1)) or the uint16 rint(65535 * clip(v, 0, 1)) of the fused slice-apply
+// kernels (slice_rows.cuh).  The pyramid's last upsample-and-add writes its result with it.
+template <int kOut>
+__global__ void __launch_bounds__(256)
+resize_bilinear_ac_quantize_kernel(const float* __restrict__ in, const float* __restrict__ add,
+                                   void* __restrict__ out, int H, int W, int C, int OH, int OW,
+                                   float sy, float sx, long long total) {
+  for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
        e += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(e % C);
-    const int ox = static_cast<int>((e / C) % OW);
-    const int oy = static_cast<int>((e / (static_cast<long long>(C) * OW)) % OH);
-    const int b = static_cast<int>(e / (static_cast<long long>(C) * OW * OH));
-    const AcTaps ty = ac_taps(oy, sy, H), tx = ac_taps(ox, sx, W);
-    const int y0 = ty.lo, y1 = ty.hi, x0 = tx.lo, x1 = tx.hi;
-    const float fy = ty.frac, fx = tx.frac;
-    const float* img = in + static_cast<size_t>(b) * H * W * C;
-    const float tl = __ldg(img + (static_cast<size_t>(y0) * W + x0) * C + c);
-    const float tr = __ldg(img + (static_cast<size_t>(y0) * W + x1) * C + c);
-    const float bl = __ldg(img + (static_cast<size_t>(y1) * W + x0) * C + c);
-    const float br = __ldg(img + (static_cast<size_t>(y1) * W + x1) * C + c);
-    const float top = tl + (tr - tl) * fx;
-    const float bot = bl + (br - bl) * fx;
-    float v = top + (bot - top) * fy;
-    if (add) v += __ldg(add + e);
-    out[e] = v;
+    const float v = resize_ac_value(in, add, H, W, C, OH, OW, sy, sx, e);
+    if constexpr (kOut == kPxU8)
+      static_cast<unsigned char*>(out)[e] = static_cast<unsigned char>(float_to_u8(v));
+    else
+      static_cast<unsigned short*>(out)[e] = static_cast<unsigned short>(float_to_u16(v));
   }
 }
 
@@ -205,3 +231,54 @@ extern "C" int hdrnet_lowres_nearest_f32(const void* image, int fmt, float* lowr
   }
   return static_cast<int>(cudaGetLastError());
 }
+
+// ---- pieces of the whole-model C path (model.cu) ---------------------------------------------
+namespace hdrnet_b200 {
+
+// img_as_float of a whole image (code_to_float per element): the float full-resolution image the
+// pyramid's levels are resized from, bit-exact where models.image_to_float is not (row f-11).
+template <int kFmt>
+__global__ void __launch_bounds__(256)
+image_to_float_kernel(const void* __restrict__ image, float* __restrict__ out, long long total) {
+  for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
+       e += static_cast<long long>(gridDim.x) * blockDim.x)
+    out[e] = code_to_float<kFmt>(image, e);
+}
+
+static unsigned elementwise_blocks(long long total) {
+  const long long blocks = (total + 255) / 256;
+  return static_cast<unsigned>(blocks > 132LL * 32 ? 132LL * 32 : blocks);
+}
+
+// `total` uint8 / uint16 code values -> float32.
+int launch_image_to_float(const void* image, int fmt, float* out, long long total, cudaStream_t st) {
+  if (total == 0) return HDRNET_OK;
+  if (fmt == HDRNET_PX_U8)
+    image_to_float_kernel<HDRNET_PX_U8><<<elementwise_blocks(total), 256, 0, st>>>(image, out, total);
+  else if (fmt == HDRNET_PX_U16)
+    image_to_float_kernel<HDRNET_PX_U16><<<elementwise_blocks(total), 256, 0, st>>>(image, out, total);
+  else
+    return HDRNET_E_UNSUPPORTED;
+  return static_cast<int>(cudaGetLastError());
+}
+
+// hdrnet_resize_bilinear_f32(in, add, ...) written through the uint8 or uint16 epilogue.
+int launch_resize_quantize(const float* in, const float* add, void* out, int out_fmt, int B, int H,
+                           int W, int C, int OH, int OW, cudaStream_t st) {
+  if (B < 0 || H < 1 || W < 1 || C < 1 || OH < 1 || OW < 1) return HDRNET_E_BAD_SHAPE;
+  const long long total = static_cast<long long>(B) * OH * OW * C;
+  if (total == 0) return HDRNET_OK;
+  if (!in || !out) return HDRNET_E_NULL_POINTER;
+  const float sy = (OH > 1) ? static_cast<float>(H - 1) / static_cast<float>(OH - 1) : 0.0f;
+  const float sx = (OW > 1) ? static_cast<float>(W - 1) / static_cast<float>(OW - 1) : 0.0f;
+  const unsigned nb = elementwise_blocks(total);
+  if (out_fmt == HDRNET_PX_U8)
+    resize_bilinear_ac_quantize_kernel<HDRNET_PX_U8><<<nb, 256, 0, st>>>(in, add, out, H, W, C, OH, OW, sy, sx, total);
+  else if (out_fmt == HDRNET_PX_U16)
+    resize_bilinear_ac_quantize_kernel<HDRNET_PX_U16><<<nb, 256, 0, st>>>(in, add, out, H, W, C, OH, OW, sy, sx, total);
+  else
+    return HDRNET_E_UNSUPPORTED;
+  return static_cast<int>(cudaGetLastError());
+}
+
+}  // namespace hdrnet_b200

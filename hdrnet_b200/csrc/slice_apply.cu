@@ -43,6 +43,7 @@
 #include <cstdint>
 #include <cstdlib>
 #include <mutex>
+#include <new>
 #include <vector>
 
 #include "slice_rows.cuh"
@@ -902,7 +903,10 @@ static int launch_tma(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream, 
 // whole workspace, not the part a call uses, so one entry serves every shape.  An entry remembers
 // an event recorded after the last launch that uses it; an evicted texture is destroyed only once
 // that event has completed (else it waits in a graveyard that later calls drain): a texture object
-// is never destroyed under a kernel that may still fetch through it.  This cache is the library's
+// is never destroyed under a kernel that may still fetch through it.  A call that a CUDA graph is
+// capturing takes no cached texture (a graph replays long after any event recorded at capture, and
+// the cache may have evicted the entry by then): it creates a texture of its own that the graph owns
+// (graph_slab_texture).  This cache and the list of textures released by graphs are the library's
 // only process-wide state.
 struct TexCacheEntry { const void* ptr; size_t bytes; int dev; cudaTextureObject_t tex; cudaEvent_t last_use; };
 constexpr int kTexCacheEntries = 16;
@@ -910,6 +914,11 @@ static std::mutex g_tex_mutex;
 static TexCacheEntry g_tex_cache[kTexCacheEntries];
 static int g_tex_next = 0;
 static std::vector<TexCacheEntry> g_tex_graveyard;
+// Textures whose graphs are gone.  Filled by user-object destructors, which may not call CUDA and
+// may run on a driver thread, so this list has a lock of its own that is never held across a CUDA
+// call; the next texture request destroys them.
+static std::mutex g_graph_tex_mutex;
+static std::vector<cudaTextureObject_t> g_graph_tex_released;
 
 static void drain_tex_graveyard_locked() {
   for (size_t i = 0; i < g_tex_graveyard.size();) {
@@ -926,15 +935,16 @@ static void drain_tex_graveyard_locked() {
   (void)cudaGetLastError();   // cudaErrorNotReady of a pending event is not an error of this call
 }
 
-// The texture over [ws, ws + bytes); `*use` must be recorded on the launch stream after the last
-// kernel of this call that fetches through it (mark_texture_used).
-static int get_slab_texture(const float* ws, size_t bytes, cudaTextureObject_t* out, cudaEvent_t* use) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lock(g_tex_mutex);
-  if (!g_tex_graveyard.empty()) drain_tex_graveyard_locked();
-  for (auto& e : g_tex_cache)
-    if (e.tex && e.ptr == ws && e.bytes == bytes && e.dev == dev) { *out = e.tex; *use = e.last_use; return 0; }
+static void destroy_released_graph_textures() {
+  std::vector<cudaTextureObject_t> released;
+  {
+    std::lock_guard<std::mutex> lock(g_graph_tex_mutex);
+    released.swap(g_graph_tex_released);
+  }
+  for (cudaTextureObject_t t : released) cudaDestroyTextureObject(t);
+}
+
+static int create_slab_texture(const float* ws, size_t bytes, cudaTextureObject_t* tex) {
   cudaResourceDesc rd = {};
   rd.resType = cudaResourceTypeLinear;
   rd.res.linear.devPtr = const_cast<float*>(ws);
@@ -942,14 +952,27 @@ static int get_slab_texture(const float* ws, size_t bytes, cudaTextureObject_t* 
   rd.res.linear.sizeInBytes = bytes;
   cudaTextureDesc td = {};
   td.readMode = cudaReadModeElementType;
+  *tex = 0;
+  cudaError_t err = cudaCreateTextureObject(tex, &rd, &td, nullptr);
+  if (err != cudaSuccess) (void)cudaGetLastError();   // report it from this call only: the next launch's check must not see it
+  return static_cast<int>(err);
+}
+
+// The texture over [ws, ws + bytes); `*use` must be recorded on the launch stream after the last
+// kernel of this call that fetches through it.
+static int get_slab_texture(const float* ws, size_t bytes, cudaTextureObject_t* out, cudaEvent_t* use) {
+  destroy_released_graph_textures();
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(g_tex_mutex);
+  if (!g_tex_graveyard.empty()) drain_tex_graveyard_locked();
+  for (auto& e : g_tex_cache)
+    if (e.tex && e.ptr == ws && e.bytes == bytes && e.dev == dev) { *out = e.tex; *use = e.last_use; return 0; }
   cudaTextureObject_t tex = 0;
-  cudaError_t err = cudaCreateTextureObject(&tex, &rd, &td, nullptr);
-  if (err != cudaSuccess) {
-    (void)cudaGetLastError();   // report it from this call only: the next launch's check must not see it
-    return static_cast<int>(err);
-  }
+  const int rc = create_slab_texture(ws, bytes, &tex);
+  if (rc != 0) return rc;
   cudaEvent_t ev = nullptr;
-  err = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  cudaError_t err = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
   if (err != cudaSuccess) { cudaDestroyTextureObject(tex); return static_cast<int>(err); }
   TexCacheEntry& slot = g_tex_cache[g_tex_next];
   g_tex_next = (g_tex_next + 1) % kTexCacheEntries;
@@ -958,6 +981,56 @@ static int get_slab_texture(const float* ws, size_t bytes, cudaTextureObject_t* 
   *out = tex;
   *use = ev;
   return 0;
+}
+
+// User-object destructor of a graph-owned texture: runs once the graph and every executable graph
+// made from it are destroyed and their launches have completed.
+static void release_graph_texture(void* p) {
+  cudaTextureObject_t* t = static_cast<cudaTextureObject_t*>(p);
+  {
+    std::lock_guard<std::mutex> lock(g_graph_tex_mutex);
+    g_graph_tex_released.push_back(*t);
+  }
+  delete t;
+}
+
+// The texture over [ws, ws + bytes) for a call that `graph` is capturing: created for this call and
+// owned by the graph through a user object, so it lives exactly as long as the graph can be replayed.
+static int graph_slab_texture_relaxed(const float* ws, size_t bytes, cudaGraph_t graph, cudaTextureObject_t* out) {
+  destroy_released_graph_textures();
+  cudaTextureObject_t tex = 0;
+  int rc = create_slab_texture(ws, bytes, &tex);
+  if (rc != 0) return rc;
+  cudaTextureObject_t* owned = new (std::nothrow) cudaTextureObject_t(tex);
+  if (!owned) { cudaDestroyTextureObject(tex); return static_cast<int>(cudaErrorMemoryAllocation); }
+  cudaUserObject_t obj = nullptr;
+  cudaError_t err = cudaUserObjectCreate(&obj, owned, release_graph_texture, 1, cudaUserObjectNoDestructorSync);
+  if (err != cudaSuccess) {
+    (void)cudaGetLastError();
+    delete owned;
+    cudaDestroyTextureObject(tex);
+    return static_cast<int>(err);
+  }
+  err = cudaGraphRetainUserObject(graph, obj, 1, cudaGraphUserObjectMove);
+  if (err != cudaSuccess) {
+    (void)cudaGetLastError();
+    cudaUserObjectRelease(obj, 1);   // the destructor queues the texture for destruction
+    return static_cast<int>(err);
+  }
+  *out = tex;
+  return 0;
+}
+
+// Texture creation counts as an unsafe call while a capture in the global mode is in progress (the
+// mode torch.cuda.graph uses), which would invalidate the capture; it does not touch any stream, so
+// this thread makes it in the relaxed mode and restores its mode after.
+static int graph_slab_texture(const float* ws, size_t bytes, cudaGraph_t graph, cudaTextureObject_t* out) {
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  cudaError_t err = cudaThreadExchangeStreamCaptureMode(&mode);
+  if (err != cudaSuccess) { (void)cudaGetLastError(); return static_cast<int>(err); }
+  const int rc = graph_slab_texture_relaxed(ws, bytes, graph, out);
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  return rc;
 }
 
 // Guide source of a launch: an input tensor, or one of the fused per-pixel guide networks.
@@ -1196,7 +1269,15 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
   // texture-assisted forms
   a.yslab = gs.workspace;
   cudaEvent_t tex_use = nullptr;
-  rc = get_slab_texture(gs.workspace, gs.workspace_bytes, &a.slab_tex, &tex_use);
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  cudaGraph_t graph = nullptr;
+  if (cudaStreamGetCaptureInfo(stream, &capture, nullptr, &graph) != cudaSuccess) {
+    (void)cudaGetLastError();   // the launch below reports what is wrong with the stream
+    capture = cudaStreamCaptureStatusNone;
+  }
+  rc = capture == cudaStreamCaptureStatusActive
+           ? graph_slab_texture(gs.workspace, gs.workspace_bytes, graph, &a.slab_tex)
+           : get_slab_texture(gs.workspace, gs.workspace_bytes, &a.slab_tex, &tex_use);
   if (rc != 0) return rc;
   if (f.pre_pass) {   // every row's y-pre-blended slab into the workspace
     rc = launch_yblend(grid, gs.workspace, g, f.p.row_floats, stream);
@@ -1210,8 +1291,9 @@ static int launch_slice_apply_impl(const float* grid, const GuideSpec& gs, const
   } else {
     rc = launch_block_sync<kSyncTexChunks>(a, gs, stream);
   }
-  // the texture must outlive every kernel that fetches through it (get_slab_texture)
-  if (rc == 0 && cudaEventRecord(tex_use, stream) != cudaSuccess) rc = static_cast<int>(cudaGetLastError());
+  // the texture must outlive every kernel that fetches through it (get_slab_texture; a captured
+  // call's texture belongs to its graph)
+  if (rc == 0 && tex_use && cudaEventRecord(tex_use, stream) != cudaSuccess) rc = static_cast<int>(cudaGetLastError());
   return rc;
 }
 
@@ -1291,7 +1373,8 @@ const char* hdrnet_b200_error_string(int code) {
     case HDRNET_E_BAD_CHANNELS: return "grid channels do not match n_out * (n_in + has_offset)";
     case HDRNET_E_TOO_LARGE: return "extent exceeds the kernels' 32-bit index range";
     case HDRNET_E_UNSUPPORTED: return "requested kernel variant cannot run these shapes";
-    case HDRNET_E_BAD_CONTEXT: return "invalid host-path context";
+    case HDRNET_E_BAD_CONTEXT: return "invalid or destroyed context or model object, or not its device";
+    case HDRNET_E_BAD_MODEL: return "malformed frozen model (magic, version, lengths, shapes or CRC-32C)";
     default: break;
   }
   if (code > 0) return cudaGetErrorString(static_cast<cudaError_t>(code));

@@ -49,7 +49,8 @@ extern "C" {
 #define HDRNET_E_BAD_CHANNELS (-3)   /* gc != n_out * (n_in + has_offset)                  */
 #define HDRNET_E_TOO_LARGE (-4)      /* an extent does not fit the kernels' 32-bit indices */
 #define HDRNET_E_UNSUPPORTED (-5)    /* the requested variant cannot run these shapes      */
-#define HDRNET_E_BAD_CONTEXT (-6)    /* invalid / destroyed host-path context              */
+#define HDRNET_E_BAD_CONTEXT (-6)    /* invalid / destroyed context or model, wrong device */
+#define HDRNET_E_BAD_MODEL (-7)      /* malformed frozen model file                        */
 
 /* Kernel selection for the *_variant debug entry points. */
 #define HDRNET_VARIANT_AUTO 0    /* what the plain entry points use                        */
@@ -542,6 +543,60 @@ HDRNET_API int hdrnet_host_ctx_destroy(hdrnet_host_ctx* ctx);
 HDRNET_API int hdrnet_slice_apply_host_f32(hdrnet_host_ctx* ctx, const float* grid, const float* guide,
                                 const float* input, float* out, int B, int H, int W, int gh,
                                 int gw, int gd, int n_in, int n_out, int has_offset);
+
+/*
+ * A whole trained model (HDRNetCurves, HDRNetPointwiseNNGuide or HDRNetGaussianPyrNN) from its frozen
+ * model file (hdrnet_b200.checkpoint.freeze_model; the layout is documented in csrc/model.cu and
+ * DESIGN.md row f-12): the C counterpart of models.*.inference_image, running the same kernels chosen
+ * by the same rules, so its results are bit for bit that path's -- except the pyramid from uint8 /
+ * uint16 pixels, whose full-resolution image is converted with the bit-exact img_as_float here where
+ * models.image_to_float divides through torch (DESIGN.md row f-11): there the results are bit for bit
+ * HDRNetGaussianPyrNN.inference on the host's img_as_float, quantised as inference_image quantises.
+ *
+ * hdrnet_model_create: checks the whole host blob (magic, format version, lengths, every array's
+ *   shape against the hyperparameters, CRC-32C) before any CUDA call -- HDRNET_E_BAD_MODEL for any
+ *   fault -- then uploads the weights to the CURRENT device and packs the tensor-core conv weights
+ *   once.  The only call that allocates device memory (and it synchronises).  The blob may be freed
+ *   after the call.
+ * hdrnet_model_destroy: frees the object (after work still reading its weights); any later use of
+ *   the handle returns HDRNET_E_BAD_CONTEXT.
+ * hdrnet_model_info: the model kind (HDRNET_MODEL_*) and hyperparameters; NULL outputs are skipped.
+ * hdrnet_model_workspace_bytes: the workspace hdrnet_model_run_px needs for B images of H x W in
+ *   in_fmt -> out_fmt (any base address; 0 for a bad handle or format).
+ * hdrnet_model_run_px: image [B,H,W,3] in in_fmt -> out [B,H,W,3] in out_fmt (HDRNET_PX_*, device
+ *   pointers): the network input is lowres_image [B,SH,SW,3] in lowres_fmt when not NULL, else the
+ *   image itself, resized nearest-neighbour to net_input_size (hdrnet_lowres_nearest_f32).  Every
+ *   intermediate lives in the lent workspace, which is scratch (undefined after the call, never read
+ *   before being written).  The call allocates no memory, never synchronises and launches only on
+ *   `stream`, so it can be captured in a CUDA graph; calls on different streams with different
+ *   workspaces may run concurrently.  The texture-assisted forms (from 2 Mi pixels per call) fetch the
+ *   slab through a texture object over the workspace: outside a capture the library creates it on a
+ *   workspace's first use and caches it; under a capture the call creates one that the graph owns and
+ *   that is destroyed only after the graph and its executable graphs are gone, so a graph replays
+ *   correctly however many other workspaces are lent meanwhile.  Errors, all before any launch:
+ *   HDRNET_E_BAD_CONTEXT for a
+ *   destroyed handle or a current device other than the one the model was created on;
+ *   HDRNET_E_BAD_SHAPE for a workspace smaller than hdrnet_model_workspace_bytes, negative extents,
+ *   or a pyramid image under 4 x 4; HDRNET_E_UNSUPPORTED for an unknown format or a uint16 `out`
+ *   overlapping `image`.  B * H * W == 0 succeeds without launching.
+ */
+#define HDRNET_MODEL_CURVES 0
+#define HDRNET_MODEL_POINTWISE_NN 1
+#define HDRNET_MODEL_GAUSSIAN_PYR_NN 2
+
+typedef struct hdrnet_model hdrnet_model;
+
+HDRNET_API int hdrnet_model_create(const void* blob, size_t bytes, hdrnet_model** model);
+HDRNET_API int hdrnet_model_destroy(hdrnet_model* model);
+HDRNET_API int hdrnet_model_info(const hdrnet_model* model, int* kind, int* net_input_size,
+                                 int* spatial_bin, int* luma_bins, int* channel_multiplier,
+                                 int* guide_width);
+HDRNET_API size_t hdrnet_model_workspace_bytes(const hdrnet_model* model, int B, int H, int W,
+                                               int in_fmt, int out_fmt);
+HDRNET_API int hdrnet_model_run_px(const hdrnet_model* model, const void* image, int in_fmt,
+                                   const void* lowres_image, int lowres_fmt, int SH, int SW,
+                                   void* out, int out_fmt, int B, int H, int W, void* workspace,
+                                   size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 } /* extern "C" */

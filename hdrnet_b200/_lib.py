@@ -101,10 +101,37 @@ SIGNATURES = {
     # (model, image, in_fmt, lowres, lowres_fmt, SH, SW, out, out_fmt, B, H, W, ws, bytes, stream)
     "hdrnet_model_run_px": (_c_int, [_vp, _vp, _c_int, _vp] + [_c_int] * 3 + [_vp] + [_c_int] * 4
                             + [_vp, ctypes.c_size_t, _vp]),
+    # ragged batches: (descs, B, fmt, lowres, SH, SW, stream); (descs, B, gh, gw, gd)
+    "hdrnet_lowres_nearest_ragged_f32": (_c_int, [_vp, _c_int, _c_int, _vp, _c_int, _c_int, _vp]),
+    "hdrnet_slice_apply_ragged_workspace_bytes": (ctypes.c_size_t, [_vp] + [_c_int] * 4),
+    # (grid, descs, B, in_fmt, out_fmt, gh, gw, gd, guide params..., ws, bytes, stream)
+    "hdrnet_slice_apply_curves_ragged_px_ws": (_c_int, [_vp, _vp] + [_c_int] * 6 + [_vp] * 5
+                                               + [ctypes.c_float, _vp, ctypes.c_size_t, _vp]),
+    "hdrnet_slice_apply_nn_ragged_px_ws": (_c_int, [_vp, _vp] + [_c_int] * 6 + [_vp] * 3
+                                           + [ctypes.c_float, _c_int, _vp, ctypes.c_size_t, _vp]),
+    "hdrnet_model_workspace_bytes_ragged": (ctypes.c_size_t, [_vp, _vp] + [_c_int] * 3),
+    # (model, descs, B, in_fmt, out_fmt, lowres descs, lowres_fmt, ws, bytes, stream)
+    "hdrnet_model_run_ragged_px": (_c_int, [_vp, _vp] + [_c_int] * 3 + [_vp, _c_int, _vp, ctypes.c_size_t, _vp]),
 }
 
 # pixel storage formats (include/hdrnet_b200.h HDRNET_PX_*)
 PX_F32, PX_U8, PX_U16 = 0, 1, 2
+
+# images per launch of the ragged kernels (HDRNET_RAGGED_MAX_IMAGES): longer calls are split
+RAGGED_MAX_IMAGES = 256
+
+
+class ImageDesc(ctypes.Structure):
+    """hdrnet_image_desc: one image of a ragged batch (device pointers to [H, W, 3] buffers)."""
+    _fields_ = [("image", _vp), ("out", _vp), ("H", _c_int), ("W", _c_int)]
+
+
+def image_descs(images, outs=None):
+    """A ctypes array of hdrnet_image_desc for CUDA tensors [H_i, W_i, 3] (and their outputs)."""
+    arr = (ImageDesc * max(len(images), 1))()
+    for i, im in enumerate(images):
+        arr[i] = ImageDesc(im.data_ptr(), 0 if outs is None else outs[i].data_ptr(), im.shape[0], im.shape[1])
+    return arr
 
 
 class TrainSample(ctypes.Structure):

@@ -4,6 +4,7 @@ arguments and flags, hdrnet/bin/run.py:219-238):
 
     python -m hdrnet_b200.bin.run <checkpoint_dir> <input> <output> [--lowres_input X]
                                   [--hdrp] [--debug] [--limit N] [--output_bit_depth {8,16}]
+                                  [--batch_size N]
 
 ``checkpoint_dir`` holds ``weights.npz`` (reference variable names, '/' written as '__') and
 ``params.json`` (the model_params the reference stores as graph constants, train.py:60-63,
@@ -20,6 +21,11 @@ Host-side pre/post processing follows the reference (run.py:139-190):
 PNG, rint(65535 * clip(out, 0, 1)) from the same fused kernel, instead of the 8-bit cast that drops
 half the bits a model trained on 16-bit targets produces.  The default, 8, writes what the reference
 writes; the ``--debug`` pictures are 8-bit either way.
+
+``--batch_size N`` is another addition: with N > 1, N consecutive files of the listing (of one pixel
+dtype) go through one ``inference_images`` call, whatever their sizes, and each file's PNG holds the
+same bytes as with N = 1 (the default, which runs one ``inference_image`` call per file as before).
+``--limit`` still counts files; ``--debug`` needs N = 1.
 """
 from __future__ import annotations
 
@@ -156,10 +162,38 @@ def debug_images(im_rgb: np.ndarray, coeffs: np.ndarray, guides: list, multiscal
     return out
 
 
+def _rgb3(im: np.ndarray) -> np.ndarray:
+    """process()'s channel handling: grey to three channels, alpha dropped."""
+    if im.ndim == 2:
+        im = np.repeat(im[..., None], 3, axis=2)
+    return np.ascontiguousarray(im[:, :, :3])
+
+
+def process_batch(mdl, params, ims: list, lowres: list, out_dtype=torch.uint8) -> list:
+    """Several decoded images of one dtype, each of its own size, through one ``inference_images``
+    call; ``lowres`` holds each image's network-input image or None (the image itself).  Returns
+    one HxWx3 array per image, the bytes ``process`` returns for it."""
+    def to_dev(a):
+        if a.dtype not in (np.uint8, np.uint16):
+            a = a.astype(np.float32)
+        return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+    full = [to_dev(_rgb3(im)) for im in ims]
+    low = None
+    if any(lo is not None for lo in lowres):
+        low = [full[i] if lo is None else to_dev(_rgb3(lo)) for i, lo in enumerate(lowres)]
+    return [o.cpu().numpy() for o in mdl.inference_images(full, params, lowres_images=low, out_dtype=out_dtype)]
+
+
 def main(args):
-    import cv2
     # callers that build the namespace themselves may leave the flag out: 8, as the parser's default
     out_dtype = OUTPUT_DTYPES[int(getattr(args, "output_bit_depth", 8))]
+    batch_size = int(getattr(args, "batch_size", 1))
+    if batch_size < 1:
+        raise ValueError(f"--batch_size must be at least 1, got {batch_size}")
+    if batch_size > 1 and args.debug:
+        raise ValueError("--debug writes one image's collections: it needs --batch_size 1")
+    import cv2
     params, _ = load_checkpoint(args.checkpoint_dir)
     mdl = getattr(models, params["model_name"])                     # run.py:82-85
     params["debug"] = bool(args.debug)
@@ -167,6 +201,9 @@ def main(args):
     if args.limit is not None:
         paths = paths[:args.limit]
     os.makedirs(args.output, exist_ok=True)
+    if batch_size > 1:
+        _run_batches(cv2, mdl, params, args, paths, batch_size, out_dtype)
+        return
     for i, path in enumerate(paths):
         log.info("Processing %s (%d/%d)", path, i + 1, len(paths))
         bgr = cv2.imread(path, -1)
@@ -193,6 +230,36 @@ def main(args):
                 cv2.imwrite(os.path.join(args.output, name + fname), img)
 
 
+def _run_batches(cv2, mdl, params, args, paths, batch_size, out_dtype):
+    """main() with --batch_size > 1: batch_size consecutive files per inference_images call (split
+    where the pixel dtype changes, since one call takes one dtype)."""
+    for start in range(0, len(paths), batch_size):
+        group = []
+        for j, path in enumerate(paths[start:start + batch_size]):
+            log.info("Processing %s (%d/%d)", path, start + j + 1, len(paths))
+            bgr = cv2.imread(path, -1)
+            if bgr is None:
+                log.warning("could not read %s", path)
+                continue
+            rgb = bgr[:, :, :3][:, :, ::-1] if bgr.ndim == 3 else bgr   # run.py:150
+            if args.hdrp and rgb.dtype == np.uint16:
+                log.info("Using HDR+ hack for uint16 input. Assuming input white level is 32767.")
+            low_u = None
+            if args.lowres_input is not None:
+                lb = cv2.imread(os.path.join(args.lowres_input, os.path.basename(path)), -1)
+                low_u = lb[:, :, :3][:, :, ::-1] if lb is not None and lb.ndim == 3 else lb
+            group.append((path, rgb, low_u))
+        while group:
+            n = 1
+            while n < len(group) and group[n][1].dtype == group[0][1].dtype:
+                n += 1
+            run, group = group[:n], group[n:]
+            outs = process_batch(mdl, params, [g[1] for g in run], [g[2] for g in run], out_dtype)
+            for (path, _, _), out_q in zip(run, outs):
+                name = os.path.splitext(os.path.basename(path))[0]
+                cv2.imwrite(os.path.join(args.output, name + ".png"), out_q[:, :, ::-1])
+
+
 # --output_bit_depth -> the dtype inference_image returns and cv2.imwrite stores
 OUTPUT_DTYPES = {8: torch.uint8, 16: torch.uint16}
 
@@ -209,6 +276,8 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--limit", type=int)
     parser.add_argument("--output_bit_depth", type=int, choices=sorted(OUTPUT_DTYPES), default=8,
                         help="8: uint8 PNGs, as the reference writes; 16: 16-bit PNGs, rint(65535 * clip)")
+    parser.add_argument("--batch_size", type=int, default=1,
+                        help="files per model call; images of different sizes batch together (default 1)")
     parser.set_defaults(hdrp=False, debug=False)
     return parser
 

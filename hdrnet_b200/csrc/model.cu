@@ -31,6 +31,7 @@
 #include "common.cuh"
 
 namespace hdrnet_b200 {
+int validate_ragged(const hdrnet_image_desc* images, int B, int in_fmt, int out_fmt, bool need_out, int min_hw);
 int launch_image_to_float(const void* image, int fmt, float* out, long long total, cudaStream_t st);
 int launch_resize_quantize(const float* in, const float* add, void* out, int out_fmt, int B, int H,
                            int W, int C, int OH, int OW, cudaStream_t st);
@@ -264,6 +265,40 @@ void layout(const hdrnet_model* m, int B, int H, int W, int in_fmt, int out_fmt,
   l->end = c.off;
 }
 
+// The workspace of a ragged batch (hdrnet_model_run_ragged_px): the network input, grids and
+// activations for all B images; for the pyramid, each level's coefficient rows for all B images and
+// the per-image intermediates of pyramid_fullres sized for the largest image at each level (the
+// images run one after the other on the stream, so they share them).
+void layout_ragged(const hdrnet_model* m, const hdrnet_image_desc* images, int B, int in_fmt, uintptr_t base,
+                   Layout* l) {
+  const Hyper& h = m->h;
+  const size_t f = sizeof(float);
+  Carver c{base};
+  *l = Layout{};
+  l->lowres = c.take(static_cast<size_t>(B) * h.S * h.S * 3 * f);
+  l->grid = c.take(static_cast<size_t>(B) * h.sb * h.sb * h.gd * n_out_of(h.kind) * 4 * f);
+  l->acts_bytes = hdrnet_coefficients_scratch_bytes(B, h.S, h.sb, h.gd, h.cm, n_out_of(h.kind), 4);
+  l->acts = c.take(l->acts_bytes);
+  if (h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN) {
+    size_t lp[3] = {0, 0, 0};
+    for (int i = 0; i < B; ++i) {
+      const int H = images[i].H, W = images[i].W;
+      lp[0] = std::max(lp[0], static_cast<size_t>(H) * W);
+      lp[1] = std::max(lp[1], static_cast<size_t>(H / 2) * (W / 2));
+      lp[2] = std::max(lp[2], static_cast<size_t>(H / 4) * (W / 4));
+    }
+    if (in_fmt != HDRNET_PX_F32) l->full = c.take(lp[0] * 3 * f);
+    for (int i = 0; i < 3; ++i) {
+      if (i > 0) l->lvl[i] = c.take(lp[i] * 3 * f);
+      l->coef[i] = c.take(static_cast<size_t>(B) * h.sb * h.sb * h.gd * 12 * f);
+      l->lvl_out[i] = c.take(lp[i] * 3 * f);
+      l->lvl_gmap[i] = c.take(lp[i] * f);
+    }
+    l->cur1 = c.take(lp[1] * 3 * f);
+  }
+  l->end = c.off;
+}
+
 // hdrnet_ops._texture_form_runs: AUTO runs a texture-assisted form from 2 Mi pixels on when lent
 // the slab workspace, and only then does models' fused slice-apply lend it.
 bool texture_form_runs(int B, int H, int W, int gd, int sb) {
@@ -359,6 +394,38 @@ split_level_rows_kernel(const float* __restrict__ coeffs, float* __restrict__ c0
     float* dst = level == 0 ? c0 : (level == 1 ? c1 : c2);
     dst[cell * 12 + r % 12] = coeffs[e];
   }
+}
+
+// HDRNetGaussianPyrNN.inference_image after the coefficients: the float image, its two smaller
+// levels, one fused slice-apply per level with its three coefficient rows `coef` (level il's rows
+// [B, sb, sb, gd, 12]), coarse-to-fine upsample-and-add.  `l` holds the intermediates for B x H x W.
+int pyramid_fullres(const hdrnet_model* m, const Layout& l, const float* const coef[3], const void* image,
+                    int in_fmt, void* out, int out_fmt, int B, int H, int W, cudaStream_t st) {
+  const long long npx = static_cast<long long>(B) * H * W;
+  int rc = HDRNET_OK;
+  const float* lvl[3] = {static_cast<const float*>(image), l.lvl[1], l.lvl[2]};
+  if (in_fmt != HDRNET_PX_F32) {
+    rc = hdrnet_b200::launch_image_to_float(image, in_fmt, l.full, npx * 3, st);
+    lvl[0] = l.full;
+  }
+  const int hs[3] = {H, H / 2, H / 4}, ws[3] = {W, W / 2, W / 4};
+  for (int i = 1; i < 3 && !rc; ++i)
+    rc = hdrnet_resize_bilinear_f32(lvl[i - 1], nullptr, l.lvl[i], B, hs[i - 1], ws[i - 1], 3, hs[i], ws[i], st);
+  for (int il = 0; il < 3 && !rc; ++il) {
+    const int src = 2 - il;   // reversed(zip(lvls, guides)): the coarsest level takes rows 0..2
+    float* gmap = fused_row_kernel_takes(ws[src], lvl[src], l.lvl_out[src], coef[il]) ? nullptr : l.lvl_gmap[src];
+    rc = slice_apply(m, src, coef[il], lvl[src], HDRNET_PX_F32, l.lvl_out[src], HDRNET_PX_F32, gmap, B, hs[src],
+                     ws[src], nullptr, 0, st);
+    if (rc || il == 0) continue;
+    const float* current = il == 1 ? l.lvl_out[2] : l.cur1;
+    if (il == 1)
+      rc = hdrnet_resize_bilinear_f32(current, l.lvl_out[1], l.cur1, B, hs[2], ws[2], 3, hs[1], ws[1], st);
+    else if (out_fmt == HDRNET_PX_F32)
+      rc = hdrnet_resize_bilinear_f32(current, l.lvl_out[0], static_cast<float*>(out), B, hs[1], ws[1], 3, H, W, st);
+    else
+      rc = hdrnet_b200::launch_resize_quantize(current, l.lvl_out[0], out, out_fmt, B, hs[1], ws[1], 3, H, W, st);
+  }
+  return rc;
 }
 
 bool valid_fmt(int f) { return f == HDRNET_PX_F32 || f == HDRNET_PX_U8 || f == HDRNET_PX_U16; }
@@ -530,27 +597,63 @@ int hdrnet_model_run_px(const hdrnet_model* m, const void* image, int in_fmt, co
   split_level_rows_kernel<<<static_cast<unsigned>(std::min<long long>((cells * 36 + 255) / 256, 132LL * 32)), 256, 0,
                             st>>>(l.grid, l.coef[0], l.coef[1], l.coef[2], cells * 36);
   rc = static_cast<int>(cudaGetLastError());
-  const float* lvl[3] = {static_cast<const float*>(image), l.lvl[1], l.lvl[2]};
-  if (!rc && in_fmt != HDRNET_PX_F32) {
-    rc = hdrnet_b200::launch_image_to_float(image, in_fmt, l.full, npx * 3, st);
-    lvl[0] = l.full;
+  if (rc) return rc;
+  const float* coef[3] = {l.coef[0], l.coef[1], l.coef[2]};
+  return pyramid_fullres(m, l, coef, image, in_fmt, out, out_fmt, B, H, W, st);
+}
+
+size_t hdrnet_model_workspace_bytes_ragged(const hdrnet_model* m, const hdrnet_image_desc* images, int B, int in_fmt,
+                                           int out_fmt) {
+  if (!is_live(m) || !valid_fmt(in_fmt) || !valid_fmt(out_fmt) || B < 0 || (B > 0 && !images)) return 0;
+  for (int i = 0; i < B; ++i)
+    if (images[i].H <= 0 || images[i].W <= 0) return 0;
+  Layout l;
+  layout_ragged(m, images, B, in_fmt, 0, &l);
+  return l.end + kAlign;   // + kAlign: any base is aligned up to kAlign
+}
+
+int hdrnet_model_run_ragged_px(const hdrnet_model* m, const hdrnet_image_desc* images, int B, int in_fmt,
+                               int out_fmt, const hdrnet_image_desc* lowres, int lowres_fmt, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  if (!is_live(m)) return HDRNET_E_BAD_CONTEXT;
+  int dev = -1;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev != m->device) return HDRNET_E_BAD_CONTEXT;
+  if (!valid_fmt(in_fmt) || !valid_fmt(out_fmt) || (lowres && !valid_fmt(lowres_fmt))) return HDRNET_E_UNSUPPORTED;
+  const bool pyr = m->h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN;
+  int rc = hdrnet_b200::validate_ragged(images, B, in_fmt, out_fmt, true, pyr ? 4 : 1);
+  if (rc != HDRNET_OK || B == 0) return rc;
+  if (lowres && (rc = hdrnet_b200::validate_ragged(lowres, B, lowres_fmt, out_fmt, false, 1)) != HDRNET_OK) return rc;
+  if (!workspace) return HDRNET_E_NULL_POINTER;
+  if (workspace_bytes < hdrnet_model_workspace_bytes_ragged(m, images, B, in_fmt, out_fmt)) return HDRNET_E_BAD_SHAPE;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Hyper& h = m->h;
+  Layout l;
+  layout_ragged(m, images, B, in_fmt, align_up(reinterpret_cast<uintptr_t>(workspace), kAlign), &l);
+
+  rc = hdrnet_lowres_nearest_ragged_f32(lowres ? lowres : images, B, lowres ? lowres_fmt : in_fmt, l.lowres, h.S,
+                                        h.S, st);
+  if (!rc) rc = coefficients(m, l.lowres, l.grid, l.acts, l.acts_bytes, B, st);
+  if (rc) return rc;
+  if (!pyr) {
+    if (h.kind == HDRNET_MODEL_CURVES)
+      return hdrnet_slice_apply_curves_ragged_px_ws(l.grid, images, B, in_fmt, out_fmt, h.sb, h.sb, h.gd, m->ccm,
+                                                    m->ccm_bias, m->shifts, m->slopes, m->mix, m->mix_bias, nullptr,
+                                                    0, st);
+    const NNGuideHost& g = m->nn[0];
+    return hdrnet_slice_apply_nn_ragged_px_ws(l.grid, images, B, in_fmt, out_fmt, h.sb, h.sb, h.gd, g.w1, g.b1, g.w2,
+                                              g.b2, g.feats, nullptr, 0, st);
   }
-  const int hs[3] = {H, H / 2, H / 4}, ws[3] = {W, W / 2, W / 4};
-  for (int i = 1; i < 3 && !rc; ++i)
-    rc = hdrnet_resize_bilinear_f32(lvl[i - 1], nullptr, l.lvl[i], B, hs[i - 1], ws[i - 1], 3, hs[i], ws[i], st);
-  for (int il = 0; il < 3 && !rc; ++il) {
-    const int src = 2 - il;   // reversed(zip(lvls, guides)): the coarsest level takes rows 0..2
-    float* gmap = fused_row_kernel_takes(ws[src], lvl[src], l.lvl_out[src], l.coef[il]) ? nullptr : l.lvl_gmap[src];
-    rc = slice_apply(m, src, l.coef[il], lvl[src], HDRNET_PX_F32, l.lvl_out[src], HDRNET_PX_F32, gmap, B, hs[src],
-                     ws[src], nullptr, 0, st);
-    if (rc || il == 0) continue;
-    const float* current = il == 1 ? l.lvl_out[2] : l.cur1;
-    if (il == 1)
-      rc = hdrnet_resize_bilinear_f32(current, l.lvl_out[1], l.cur1, B, hs[2], ws[2], 3, hs[1], ws[1], st);
-    else if (out_fmt == HDRNET_PX_F32)
-      rc = hdrnet_resize_bilinear_f32(current, l.lvl_out[0], static_cast<float*>(out), B, hs[1], ws[1], 3, H, W, st);
-    else
-      rc = hdrnet_b200::launch_resize_quantize(current, l.lvl_out[0], out, out_fmt, B, hs[1], ws[1], 3, H, W, st);
+  // the pyramid: its coefficient network ran on the whole batch; its full-resolution stages run image
+  // by image on hdrnet_model_run_px's kernels (there is no ragged form of the resizes)
+  const long long cells = static_cast<long long>(B) * h.sb * h.sb * h.gd;
+  split_level_rows_kernel<<<static_cast<unsigned>(std::min<long long>((cells * 36 + 255) / 256, 132LL * 32)), 256, 0,
+                            st>>>(l.grid, l.coef[0], l.coef[1], l.coef[2], cells * 36);
+  rc = static_cast<int>(cudaGetLastError());
+  const size_t image_cells = static_cast<size_t>(h.sb) * h.sb * h.gd * 12;
+  for (int i = 0; i < B && !rc; ++i) {
+    const float* coef[3] = {l.coef[0] + i * image_cells, l.coef[1] + i * image_cells, l.coef[2] + i * image_cells};
+    rc = pyramid_fullres(m, l, coef, images[i].image, in_fmt, images[i].out, out_fmt, 1, images[i].H, images[i].W,
+                         st);
   }
   return rc;
 }

@@ -7,6 +7,8 @@
 // identity and needs no kernel.
 #include <cuda_runtime.h>
 
+#include <algorithm>
+
 #include "hdrnet_b200.h"
 #include "slice_rows.cuh"
 
@@ -230,6 +232,63 @@ extern "C" int hdrnet_lowres_nearest_f32(const void* image, int fmt, float* lowr
       return HDRNET_E_UNSUPPORTED;
   }
   return static_cast<int>(cudaGetLastError());
+}
+
+// ---- the network input of a ragged batch (hdrnet_lowres_nearest_ragged_f32) -------------------
+namespace hdrnet_b200 {
+
+struct RaggedLowres {
+  int n;
+  struct { const void* image; int H, W; } img[HDRNET_RAGGED_MAX_IMAGES];
+};
+
+// lowres_nearest_kernel with each image's own pointer and extent: the same source index and
+// conversion per output element, so image b's rows equal that kernel's on image b alone.
+template <int kFmt>
+__global__ void __launch_bounds__(256)
+lowres_nearest_ragged_kernel(const __grid_constant__ RaggedLowres a, float* __restrict__ lowres, int SH,
+                             int SW, long long total) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
+       e += stride) {
+    const int c = static_cast<int>(e % 3);
+    const long long px = e / 3;
+    const int ox = static_cast<int>(px % SW);
+    const int oy = static_cast<int>((px / SW) % SH);
+    const int b = static_cast<int>(px / (static_cast<long long>(SW) * SH));
+    const int H = a.img[b].H, W = a.img[b].W;
+    const int iy = min(static_cast<int>((2LL * oy + 1) * H / (2LL * SH)), H - 1);
+    const int ix = min(static_cast<int>((2LL * ox + 1) * W / (2LL * SW)), W - 1);
+    lowres[e] = code_to_float<kFmt>(a.img[b].image, (static_cast<long long>(iy) * W + ix) * 3 + c);
+  }
+}
+
+int validate_ragged(const hdrnet_image_desc* images, int B, int in_fmt, int out_fmt, bool need_out, int min_hw);
+
+}  // namespace hdrnet_b200
+
+extern "C" int hdrnet_lowres_nearest_ragged_f32(const hdrnet_image_desc* images, int B, int fmt, float* lowres,
+                                                int SH, int SW, void* stream) {
+  using namespace hdrnet_b200;
+  if (SH < 1 || SW < 1) return HDRNET_E_BAD_SHAPE;
+  int rc = validate_ragged(images, B, fmt, HDRNET_PX_F32, false, 1);
+  if (rc != HDRNET_OK || B == 0) return rc;
+  if (!lowres) return HDRNET_E_NULL_POINTER;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (int c0 = 0; c0 < B; c0 += HDRNET_RAGGED_MAX_IMAGES) {
+    RaggedLowres a;
+    a.n = std::min(HDRNET_RAGGED_MAX_IMAGES, B - c0);
+    for (int i = 0; i < a.n; ++i) a.img[i] = {images[c0 + i].image, images[c0 + i].H, images[c0 + i].W};
+    const long long total = static_cast<long long>(a.n) * SH * SW * 3;
+    const unsigned nb = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 132LL * 32));
+    float* dst = lowres + static_cast<size_t>(c0) * SH * SW * 3;
+    if (fmt == HDRNET_PX_F32) lowres_nearest_ragged_kernel<HDRNET_PX_F32><<<nb, 256, 0, st>>>(a, dst, SH, SW, total);
+    else if (fmt == HDRNET_PX_U8) lowres_nearest_ragged_kernel<HDRNET_PX_U8><<<nb, 256, 0, st>>>(a, dst, SH, SW, total);
+    else lowres_nearest_ragged_kernel<HDRNET_PX_U16><<<nb, 256, 0, st>>>(a, dst, SH, SW, total);
+    rc = static_cast<int>(cudaGetLastError());
+    if (rc != HDRNET_OK) return rc;
+  }
+  return HDRNET_OK;
 }
 
 // ---- pieces of the whole-model C path (model.cu) ---------------------------------------------

@@ -54,47 +54,7 @@ namespace hdrnet_b200 {
 // Generic kernels: one thread per pixel, any n_in / n_out / alignment / width.
 // =========================================================================================
 
-struct Corners {
-  int off[8];    // float offsets of the 8 corner cells (channel 0) inside this image's grid
-  float w[8];    // trilinear weights, order (y, x, z) as the reference's loops
-};
-
-__device__ __forceinline__ Corners make_corners(const SliceGeom& g, int x, int y, float guide,
-                                                int gc) {
-  const Axis ax = spatial_axis(x, g.scale_x);
-  const Axis ay = spatial_axis(y, g.scale_y);
-  const Axis az = range_axis(guide, static_cast<float>(g.gd));
-  float wz[2];
-  smoothed_weights(az.f, wz[0], wz[1]);
-  const float wx[2] = {1.0f - ax.f, ax.f};
-  const float wy[2] = {1.0f - ay.f, ay.f};
-  Corners c;
-#pragma unroll
-  for (int dy = 0; dy < 2; ++dy) {
-    const int gyc = clampi(ay.i0 + dy, 0, g.gh - 1);
-#pragma unroll
-    for (int dx = 0; dx < 2; ++dx) {
-      const int gxc = clampi(ax.i0 + dx, 0, g.gw - 1);
-#pragma unroll
-      for (int dz = 0; dz < 2; ++dz) {
-        const int gzc = clampi(az.i0 + dz, 0, g.gd - 1);
-        const int k = dy * 4 + dx * 2 + dz;
-        c.off[k] = ((gyc * g.gw + gxc) * g.gd + gzc) * gc;
-        c.w[k] = wx[dx] * wy[dy] * wz[dz];
-      }
-    }
-  }
-  return c;
-}
-
-__device__ __forceinline__ float sample(const float* __restrict__ grid_b, const Corners& c,
-                                        int ch) {
-  float s = 0.0f;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) s = fmaf(c.w[k], __ldg(grid_b + c.off[k] + ch), s);
-  return s;
-}
-
+// Corners / make_corners / sample: slice_rows.cuh.
 // kApply = true : out[p, i] = sum_j sample(i*J + j) * (j < n_in ? input[p, j] : 1)
 // kApply = false: out[p, c] = sample(c), c < gc
 template <bool kApply>
@@ -1352,6 +1312,18 @@ int launch_slice(const float* grid, const float* guide, float* out, int B, int H
         grid, guide, nullptr, out, g, 0, 0, gc, npix);
   }
   return static_cast<int>(cudaGetLastError());
+}
+
+// Whether a single-image fused-guide call (hdrnet_slice_apply_{curves,nn}_px_ws, B = 1) on these
+// shapes and buffers runs a row-kernel form (TMA or texture-assisted: the 4-corner blend of the
+// y-pre-blended slab) rather than a per-pixel one: the ragged kernel (slice_apply_ragged.cu) runs
+// the same arithmetic per image.  mode: 1 = curves, 2 = pointwise NN.
+bool fused_call_runs_row_form(int H, int W, int gh, int gw, int gd, int mode, int in_fmt, int out_fmt,
+                              bool aligned) {
+  ApplyForm f;
+  return plan_slice_apply(make_geom(1, H, W, H, 0, gh, gw, gd), 3, 3, 1, mode, in_fmt, out_fmt, aligned, 0, 0,
+                          HDRNET_VARIANT_AUTO, &f) == HDRNET_OK &&
+         f.variant != HDRNET_VARIANT_GENERIC;
 }
 
 }  // namespace hdrnet_b200

@@ -1,8 +1,9 @@
 // slice_rows.cuh -- device code and plan / argument structs shared by the persistent row kernels
 // of the fused slice-apply (slice_apply.cu: block-synchronous form and host side;
 // slice_apply_async.cu: issuer-warp form; slice_apply_variants.cu: the opt-in negative-result
-// forms): pixel storage formats, the staged-tile accessors, the 4-corner blend + affine apply,
-// the guide sources, one thread's quad of pixels.
+// forms; slice_apply_ragged.cu: the ragged kernel): pixel storage formats, the staged-tile
+// accessors, the 4-corner blend + affine apply, the guide sources, one thread's quad of pixels, and
+// the per-pixel kernel's 8-corner gather.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -257,6 +258,33 @@ struct GuideNN {
 };
 
 
+// Four consecutive pixels from image column x: bit-exact cell indices, 4-corner blend of the
+// y-pre-blended slab row + affine apply.  The row kernels (process_quad) and the ragged kernel
+// (slice_apply_ragged.cu) share it, so both give the same bits for the same slab row.
+template <int kTexChunks>
+__device__ __forceinline__ void blend_quad(const SliceGeom& g, const float* slab, cudaTextureObject_t tex,
+                                           int tex_row, int x, const float (&gv)[4], const float (&pr)[4],
+                                           const float (&pg)[4], const float (&pb)[4], float (&o_r)[4],
+                                           float (&o_g)[4], float (&o_b)[4]) {
+  const float gd_f = static_cast<float>(g.gd);
+  const int x_stride = g.gd * kGc;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const Axis ax = spatial_axis(x + i, g.scale_x);
+    const Axis az = range_axis(gv[i], gd_f);
+    const int xo0 = clampi(ax.i0, 0, g.gw - 1) * x_stride;
+    const int xo1 = clampi(ax.i0 + 1, 0, g.gw - 1) * x_stride;
+    const int zo0 = clampi(az.i0, 0, g.gd - 1) * kGc;
+    const int zo1 = clampi(az.i0 + 1, 0, g.gd - 1) * kGc;
+    float wz0, wz1;
+    smoothed_weights(az.f, wz0, wz1);
+    const float wx1 = ax.f, wx0 = 1.0f - ax.f;
+    blend_apply<kTexChunks>(slab, tex, tex_row, xo0 + zo0, xo0 + zo1, xo1 + zo0,
+                            xo1 + zo1, wx0 * wz0, wx0 * wz1, wx1 * wz0, wx1 * wz1, pr[i], pg[i],
+                            pb[i], o_r[i], o_g[i], o_b[i]);
+  }
+}
+
 // One thread's 4 consecutive pixels (quad `q` of a staged segment): guide (staged, or computed
 // from RGB), bit-exact cell indices, 4-corner blend + affine apply, result written IN PLACE over
 // the RGB tile.  Shared by the block-synchronous and the warp-specialised row kernels.
@@ -284,6 +312,8 @@ __device__ __forceinline__ void process_quad(const TmaArgs& args, const GuideFn&
     }
   }
   float o_r[4], o_g[4], o_b[4];
+  // blend_quad's loop, kept inline here: its form compiles to the same instructions as before
+  // blend_quad existed (the ragged kernel reaches the same arithmetic through blend_quad)
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const Axis ax = spatial_axis(x0 + 4 * q + i, g.scale_x);
@@ -301,6 +331,92 @@ __device__ __forceinline__ void process_quad(const TmaArgs& args, const GuideFn&
   }
   store_quad<kOut>(out_tile, q, o_r, o_g, o_b);
   fence_proxy_async_smem();
+}
+
+// =========================================================================================
+// The one-thread-per-pixel corner gather (slice_generic_kernel, slice_apply_px_generic_kernel and
+// the ragged kernel's per-pixel form): 8 corners read from the grid in global memory.
+// =========================================================================================
+struct Corners {
+  int off[8];    // float offsets of the 8 corner cells (channel 0) inside this image's grid
+  float w[8];    // trilinear weights, order (y, x, z) as the reference's loops
+};
+
+__device__ __forceinline__ Corners make_corners(const SliceGeom& g, int x, int y, float guide,
+                                                int gc) {
+  const Axis ax = spatial_axis(x, g.scale_x);
+  const Axis ay = spatial_axis(y, g.scale_y);
+  const Axis az = range_axis(guide, static_cast<float>(g.gd));
+  float wz[2];
+  smoothed_weights(az.f, wz[0], wz[1]);
+  const float wx[2] = {1.0f - ax.f, ax.f};
+  const float wy[2] = {1.0f - ay.f, ay.f};
+  Corners c;
+#pragma unroll
+  for (int dy = 0; dy < 2; ++dy) {
+    const int gyc = clampi(ay.i0 + dy, 0, g.gh - 1);
+#pragma unroll
+    for (int dx = 0; dx < 2; ++dx) {
+      const int gxc = clampi(ax.i0 + dx, 0, g.gw - 1);
+#pragma unroll
+      for (int dz = 0; dz < 2; ++dz) {
+        const int gzc = clampi(az.i0 + dz, 0, g.gd - 1);
+        const int k = dy * 4 + dx * 2 + dz;
+        c.off[k] = ((gyc * g.gw + gxc) * g.gd + gzc) * gc;
+        c.w[k] = wx[dx] * wy[dy] * wz[dz];
+      }
+    }
+  }
+  return c;
+}
+
+__device__ __forceinline__ float sample(const float* __restrict__ grid_b, const Corners& c,
+                                        int ch) {
+  float s = 0.0f;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) s = fmaf(c.w[k], __ldg(grid_b + c.off[k] + ch), s);
+  return s;
+}
+
+// One pixel of the per-pixel fused forms, for the ragged kernel: the statements of
+// slice_apply_px_generic_kernel's loop body (which keeps its own copy: folded into this function it
+// compiles to different, if equivalent, instructions), so both give the same bits.  Guide computed
+// in registers from the pixel at element
+// offset 3 * p of `input`, 8-corner gather of image b's grid (grid_image floats each), 3x4 affine apply, result
+// stored at element offset 3 * p of `out` in kOut.
+template <class GuideFn, int kIn, int kOut>
+__device__ __forceinline__ void px_generic_pixel(const float* __restrict__ grid, long long grid_image, int b,
+                                                 const unsigned char* __restrict__ input,
+                                                 unsigned char* __restrict__ out, float* __restrict__ guide_out,
+                                                 const SliceGeom& g, int x, int y, long long p,
+                                                 const GuideFn& guide_fn) {
+  const float in[3] = {load_channel<kIn>(input, 3 * p), load_channel<kIn>(input, 3 * p + 1),
+                       load_channel<kIn>(input, 3 * p + 2)};
+  const float gv = guide_fn(in[0], in[1], in[2]);
+  if (guide_out != nullptr) guide_out[p] = gv;
+  const Corners c = make_corners(g, x, y, gv, 12);
+  const float* grid_b = grid + b * grid_image;
+  float o[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    float value = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) value = fmaf(sample(grid_b, c, i * 4 + j), in[j], value);
+    o[i] = value + sample(grid_b, c, i * 4 + 3);
+  }
+  if constexpr (kOut == kPxF32) {
+    float* op = reinterpret_cast<float*>(out) + 3 * p;
+    op[0] = o[0]; op[1] = o[1]; op[2] = o[2];
+  } else if constexpr (kOut == kPxU16) {
+    unsigned short* op = reinterpret_cast<unsigned short*>(out) + 3 * p;
+    op[0] = static_cast<unsigned short>(float_to_u16(o[0]));
+    op[1] = static_cast<unsigned short>(float_to_u16(o[1]));
+    op[2] = static_cast<unsigned short>(float_to_u16(o[2]));
+  } else {
+    out[3 * p] = static_cast<unsigned char>(float_to_u8(o[0]));
+    out[3 * p + 1] = static_cast<unsigned char>(float_to_u8(o[1]));
+    out[3 * p + 2] = static_cast<unsigned char>(float_to_u8(o[2]));
+  }
 }
 
 // Entry points of slice_apply_async.cu (non-template: the arguments select the instantiation).

@@ -12,7 +12,11 @@ results are bit for bit ``HDRNetGaussianPyrNN.inference`` on the host's img_as_f
 
 ``__call__`` takes the output and the workspace from torch's caching allocator on the current
 stream; ``run`` takes them from the caller and does nothing else on the host, so a
-``torch.cuda.CUDAGraph`` can capture it.
+``torch.cuda.CUDAGraph`` can capture it.  A list of images of different sizes (a ragged batch,
+``hdrnet_model_run_ragged_px``) goes the same two ways:
+
+    outs = model([im_4032x3024, im_3024x4032, im_1080p])   # list in, list out
+    model.run_images(images, outs, workspace)              # caller-lent buffers: capturable
 """
 from __future__ import annotations
 
@@ -22,7 +26,7 @@ import torch
 
 from . import _lib
 from .checkpoint import FROZEN_KINDS
-from .models import OUT_DTYPES, _PX_FMT, _check_image, _check_out_dtype
+from .models import OUT_DTYPES, _PX_FMT, _check_image, _check_images, _check_out_dtype
 
 
 class FrozenModel:
@@ -62,11 +66,28 @@ class FrozenModel:
         return int(_lib.load().hdrnet_model_workspace_bytes(self.handle, B, H, W, _PX_FMT[in_dtype],
                                                             _PX_FMT[out_dtype]))
 
-    def __call__(self, image: torch.Tensor, lowres_image: torch.Tensor | None = None,
-                 out_dtype=torch.uint8) -> torch.Tensor:
-        """image [B,H,W,3] uint8 / uint16 / float32 on the model's device -> [B,H,W,3] `out_dtype`
-        (uint8, uint16 or float32), as ``inference_image(image, params, lowres_image, out_dtype)``."""
+    def workspace_bytes_images(self, images, out_dtype=torch.uint8) -> int:
+        """Bytes of workspace ``run_images`` needs for this list of [H_i, W_i, 3] images."""
         _check_out_dtype(out_dtype)
+        images = _check_images(images, "images")
+        fmt = _PX_FMT[images[0].dtype] if images else _PX_FMT[torch.uint8]
+        return int(_lib.load().hdrnet_model_workspace_bytes_ragged(self.handle, _lib.image_descs(images), len(images),
+                                                                   fmt, _PX_FMT[out_dtype]))
+
+    def __call__(self, image, lowres_image=None, out_dtype=torch.uint8):
+        """image [B,H,W,3] uint8 / uint16 / float32 on the model's device -> [B,H,W,3] `out_dtype`
+        (uint8, uint16 or float32), as ``inference_image(image, params, lowres_image, out_dtype)``.
+        A list of [H_i, W_i, 3] images of one dtype (and `lowres_image` a list of as many, or None)
+        -> a list of [H_i, W_i, 3] results, as ``inference_images``."""
+        _check_out_dtype(out_dtype)
+        if isinstance(image, (list, tuple)):
+            images = _check_images(image, "images")
+            outs = [torch.empty(im.shape, dtype=out_dtype, device=im.device) for im in images]
+            if not images:
+                return outs
+            ws = torch.empty(self.workspace_bytes_images(images, out_dtype), dtype=torch.uint8,
+                             device=images[0].device)
+            return self.run_images(images, outs, ws, lowres_image)
         image = _check_image(image, "image")
         B, H, W, _ = image.shape
         out = torch.empty((B, H, W, 3), dtype=out_dtype, device=image.device)
@@ -99,6 +120,37 @@ class FrozenModel:
                 torch.cuda.current_stream(image.device).cuda_stream)
         _lib.check(rc, f"{self.model_name} (frozen)")
         return out
+
+    def run_images(self, images, outs, workspace: torch.Tensor, lowres_images=None) -> list:
+        """One ``hdrnet_model_run_ragged_px`` on the current stream: `images` a list of [H_i, W_i, 3]
+        tensors of one dtype, `outs` a list of contiguous tensors of the same shapes and one
+        OUT_DTYPES dtype, `workspace` any contiguous tensor of at least ``workspace_bytes_images``
+        bytes.  The descriptors are passed to the kernels by value, so a ``torch.cuda.CUDAGraph``
+        that captures this call replays it on whatever pixels those buffers then hold.  Returns
+        `outs`."""
+        images = _check_images(images, "images")
+        if len(outs) != len(images) or any(
+                o.dtype != outs[0].dtype or o.dtype not in OUT_DTYPES or o.shape != im.shape or not o.is_contiguous()
+                for o, im in zip(outs, images)):
+            raise ValueError("outs must be contiguous tensors of the images' shapes and one uint8 / uint16 / "
+                             "float32 dtype")
+        if not workspace.is_contiguous():
+            raise ValueError("workspace must be contiguous")
+        if not images:
+            return outs
+        low, lfmt = None, 0
+        if lowres_images is not None:
+            lowres_images = _check_images(lowres_images, "lowres_images")
+            if len(lowres_images) != len(images):
+                raise ValueError("lowres_images must hold one image per image")
+            low, lfmt = _lib.image_descs(lowres_images), _PX_FMT[lowres_images[0].dtype]
+        with torch.cuda.device(images[0].device):
+            rc = _lib.load().hdrnet_model_run_ragged_px(
+                self.handle, _lib.image_descs(images, outs), len(images), _PX_FMT[images[0].dtype],
+                _PX_FMT[outs[0].dtype], low, lfmt, workspace.data_ptr(),
+                workspace.numel() * workspace.element_size(), torch.cuda.current_stream(images[0].device).cuda_stream)
+        _lib.check(rc, f"{self.model_name} (frozen, ragged)")
+        return outs
 
     def close(self) -> None:
         """Destroy the C object (waits for work still reading its weights); later calls raise."""

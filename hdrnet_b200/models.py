@@ -440,6 +440,71 @@ def lowres_from_image(image: torch.Tensor, size: int) -> torch.Tensor:
     return low
 
 
+def _check_images(images, what: str) -> list:
+    """A ragged batch: a list of [H_i, W_i, 3] tensors of one dtype (uint8 / uint16 / float32) on one
+    CUDA device -> the list with every tensor contiguous.  Refuses before any device work."""
+    if not isinstance(images, (list, tuple)):
+        raise TypeError(f"{what} must be a list of tensors [H, W, 3]")
+    for t in images:
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{what} must hold torch.Tensors, got {type(t).__name__}")
+        if t.dtype not in _PX_FMT:
+            raise TypeError(f"{what} must be uint8, uint16 or float32, got {t.dtype}")
+        if t.dim() != 3 or t.shape[-1] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
+            raise ValueError(f"{what} must hold non-empty [H, W, 3] images, got {tuple(t.shape)}")
+    if len({t.dtype for t in images}) > 1:
+        raise TypeError(f"{what} mixes dtypes {sorted({str(t.dtype) for t in images})}: one call takes one pixel format")
+    if len({t.device for t in images}) > 1:
+        raise ValueError(f"{what} spans devices {sorted({str(t.device) for t in images})}: one call runs on one device")
+    if images and not images[0].is_cuda:
+        raise _lib.HdrnetLibraryError(f"{what} are on {images[0].device}: hdrnet_b200 has no CPU path")
+    return [t.contiguous() for t in images]
+
+
+def lowres_from_images(images: list, size: int) -> torch.Tensor:
+    """lowres_from_image of each image of a ragged batch (a list of [H_i, W_i, 3] tensors, checked by
+    _check_images) into one [B, size, size, 3] float32 batch, one launch per RAGGED_MAX_IMAGES images;
+    row i is bit for bit lowres_from_image(images[i][None], size)."""
+    dev = images[0].device
+    low = torch.empty((len(images), size, size, 3), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.load().hdrnet_lowres_nearest_ragged_f32(
+            _lib.image_descs(images), len(images), _PX_FMT[images[0].dtype], low.data_ptr(), size, size, _stream(dev))
+    _lib.check(rc, "lowres_nearest (ragged)")
+    return low
+
+
+def _slice_apply_fused_ragged(coeffs, images, guide, out_dtype):
+    """_slice_apply_fused over a ragged batch (hdrnet_slice_apply_{curves,nn}_ragged_px_ws): image i
+    with grid row i of coeffs [B,gh,gw,gd,3,4] -> a list of [H_i, W_i, 3] tensors of `out_dtype`."""
+    _, gh, gw, gd = coeffs.shape[:4]
+    dev = images[0].device
+    outs = [torch.empty(im.shape, dtype=out_dtype, device=dev) for im in images]
+    lib = _lib.load()
+    launch = lib.hdrnet_slice_apply_nn_ragged_px_ws if isinstance(guide, _NNGuide) \
+        else lib.hdrnet_slice_apply_curves_ragged_px_ws
+    with torch.cuda.device(dev):
+        rc = launch(coeffs.data_ptr(), _lib.image_descs(images, outs), len(images), _PX_FMT[images[0].dtype],
+                    _PX_FMT[out_dtype], gh, gw, gd, *guide.args, None, 0, _stream(dev))
+    _lib.check(rc, "BilateralSliceApply(fused guide, ragged)")
+    return outs
+
+
+def _ragged_inputs(images, lowres_images, out_dtype, params):
+    """The checks of inference_images: (images, network-input images) as contiguous lists."""
+    _check_out_dtype(out_dtype)
+    images = _check_images(images, "images")
+    if params.get("debug"):
+        raise ValueError("params['debug'] stores one batch's collections: run inference_image per image for them")
+    if lowres_images is None:
+        return images, images
+    lowres_images = _check_images(lowres_images, "lowres_images")
+    if len(lowres_images) != len(images):
+        raise ValueError("lowres_images must hold one image per image")
+    if images and lowres_images[0].device != images[0].device:
+        raise ValueError("lowres_images must be on the images' device")
+    return images, lowres_images
+
 def image_to_float(image: torch.Tensor) -> torch.Tensor:
     """skimage.img_as_float of a uint8 / uint16 tensor (IEEE division: the same float32)."""
     if image.dtype == torch.uint8:
@@ -955,6 +1020,29 @@ class HDRNetCurves(object):
         return cls._fullres(coeffs, image, params, out_dtype)
 
     @classmethod
+    def inference_images(cls, images, params, lowres_images=None, out_dtype=torch.uint8):
+        """``inference_image`` over a ragged batch: ``images`` is a list of CUDA [H_i, W_i, 3] tensors
+        of one dtype (uint8 / uint16 / float32), each of its own size -> a list of [H_i, W_i, 3]
+        tensors of ``out_dtype``.  The coefficient network runs once on the whole batch; the network
+        inputs and the full-resolution pass are one launch each over all the images (per
+        RAGGED_MAX_IMAGES images).  Image i's result is ``_fullres`` of grid row i, bit for bit
+        (DESIGN.md row f-13 names the one exception, float32 -> float32 images the row kernels do not
+        take).  ``lowres_images`` (a list of as many images) replaces the resized inputs.  Mixed dtypes
+        raise TypeError and mixed devices ValueError, before any device work; [] returns []."""
+        images, sources = _ragged_inputs(images, lowres_images, out_dtype, params)
+        if not images:
+            return []
+        lowres = lowres_from_images(sources, int(params["net_input_size"]))
+        coeffs = cls._coefficients(lowres, params, False)
+        return cls._fullres_images(coeffs, images, params, out_dtype)
+
+    @classmethod
+    def _fullres_images(cls, coeffs, images, params, out_dtype):
+        """_fullres over a ragged batch: one guide + slice + apply launch for all the images."""
+        prep = _prepare(_resolve_weights(params), params, images[0].device, cls._nn_guide)
+        return _slice_apply_fused_ragged(coeffs, images, prep.guides[0], out_dtype)
+
+    @classmethod
     def inference_image_host(cls, frames, params, out=None, device=None, out_dtype=torch.uint8):
         """``inference_image`` for frames that live in HOST memory (what hdrnet/bin/run.py does per
         file: load, ``sess.run``, save): uploads, the model and downloads of consecutive frames
@@ -1269,6 +1357,23 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
         if out_dtype == torch.uint8:
             return quantize_u8(out)
         return quantize_u16(out) if out_dtype == torch.uint16 else out
+
+    @classmethod
+    def _fullres_images(cls, coeffs, images, params, out_dtype):
+        """The pyramid over a ragged batch: the coefficients of all the images come from one network
+        call; the full-resolution stages (float image, level resizes, three slice-applies, upsample
+        and add) run image by image, as inference_image runs them on one image (there is no ragged
+        form of the resizes)."""
+        outs = []
+        with torch.cuda.device(images[0].device):
+            for i, image in enumerate(images):
+                out = cls._output(cls._multiscale_input(image_to_float(image[None])), None, coeffs[i:i + 1], params)
+                if out_dtype == torch.uint8:
+                    out = quantize_u8(out)
+                elif out_dtype == torch.uint16:
+                    out = quantize_u16(out)
+                outs.append(out[0])
+        return outs
 
     @classmethod
     def _multiscale_input(cls, fullres_input):

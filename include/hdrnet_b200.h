@@ -598,6 +598,75 @@ HDRNET_API int hdrnet_model_run_px(const hdrnet_model* model, const void* image,
                                    void* out, int out_fmt, int B, int H, int W, void* workspace,
                                    size_t workspace_bytes, void* stream);
 
+/*
+ * Ragged batches: B images of different sizes in one call (a photo collection: 4032 x 3024 next to
+ * 3024 x 4032 next to a 1080p frame).  `images` is a HOST array of B descriptors of device buffers
+ * [H, W, 3]; the library reads it before the call returns and passes it to the kernels in their
+ * parameter blocks, so a CUDA graph that captures the call keeps its own copy and a replay never
+ * reads host memory.  One kernel launch takes at most HDRNET_RAGGED_MAX_IMAGES images; a longer
+ * call is split into launches of that many inside the library.  The pixel format is one per call.
+ * Errors, all before any launch: HDRNET_E_NULL_POINTER for a NULL descriptor array (B > 0), image,
+ * output or grid; HDRNET_E_BAD_SHAPE for B < 0, H or W <= 0, gh / gw / gd < 1 or a short
+ * workspace; HDRNET_E_UNSUPPORTED for an unknown format or a uint16 output overlapping any input
+ * (or the grid).  B == 0 succeeds without launching.
+ *
+ * hdrnet_lowres_nearest_ragged_f32: hdrnet_lowres_nearest_f32 per image (out unused) into one
+ *   lowres [B, SH, SW, 3]: image i's rows are bit for bit that call on image i alone.
+ * hdrnet_slice_apply_{curves,nn}_ragged_px_ws: hdrnet_slice_apply_{curves,nn}_px_ws per image, in
+ *   one launch: image i reads grid row i of grid [B, gh, gw, gd, 12] and has its own cell scales
+ *   (gw / W_i, gh / H_i); the launch's rows are handed out across the GPU as one range, so a small
+ *   image does not leave SMs idle behind a large one.  Each image runs the per-pixel arithmetic of
+ *   the form the single-image call takes for it (the row kernels' 4-corner blend of the slab, or the
+ *   per-pixel kernel's 8-corner gather), so its result is bit for bit that call's -- except a
+ *   float32 -> float32 image the row kernels do not take at W >= 64, where the single-image call runs
+ *   the guide kernel and then the any-shape row kernel, whose apply sums in another order (equal to
+ *   within float32 rounding; DESIGN.md row f-13).  No guide map is written.
+ * hdrnet_slice_apply_ragged_workspace_bytes: the workspace those calls need: 0 (the slab rows stay
+ *   in shared memory; no texture objects); the workspace arguments are accepted and unused.
+ * hdrnet_model_workspace_bytes_ragged / hdrnet_model_run_ragged_px: hdrnet_model_run_px for a
+ *   ragged batch (each descriptor's `out` receives that image's result).  `lowres` is NULL or B
+ *   descriptors of network-input images (their `out` unused) in lowres_fmt.  The coefficient network
+ *   runs once on the whole batch; curves and pointwise-NN models then run one ragged lowres launch
+ *   and one ragged slice-apply launch per HDRNET_RAGGED_MAX_IMAGES images; the pyramid runs its
+ *   full-resolution stages image by image on the kernels of hdrnet_model_run_px.  Same rules as
+ *   hdrnet_model_run_px: no allocation, no synchronisation, capturable, every error before any
+ *   launch (HDRNET_E_BAD_SHAPE also for a pyramid image under 4 x 4).
+ */
+#define HDRNET_RAGGED_MAX_IMAGES 256
+
+typedef struct hdrnet_image_desc {
+  const void* image;   /* [H, W, 3] input pixels, device memory */
+  void* out;           /* [H, W, 3] result, device memory       */
+  int H, W;
+} hdrnet_image_desc;
+
+HDRNET_API int hdrnet_lowres_nearest_ragged_f32(const hdrnet_image_desc* images, int B, int fmt,
+                                                float* lowres, int SH, int SW, void* stream);
+HDRNET_API size_t hdrnet_slice_apply_ragged_workspace_bytes(const hdrnet_image_desc* images, int B,
+                                                            int gh, int gw, int gd);
+HDRNET_API int hdrnet_slice_apply_curves_ragged_px_ws(const float* grid,
+                                                      const hdrnet_image_desc* images, int B,
+                                                      int in_fmt, int out_fmt, int gh, int gw,
+                                                      int gd, const float* ccm,
+                                                      const float* ccm_bias, const float* shifts,
+                                                      const float* slopes, const float* mix,
+                                                      float mix_bias, void* workspace,
+                                                      size_t workspace_bytes, void* stream);
+HDRNET_API int hdrnet_slice_apply_nn_ragged_px_ws(const float* grid, const hdrnet_image_desc* images,
+                                                  int B, int in_fmt, int out_fmt, int gh, int gw,
+                                                  int gd, const float* w1, const float* b1,
+                                                  const float* w2, float b2, int feats,
+                                                  void* workspace, size_t workspace_bytes,
+                                                  void* stream);
+HDRNET_API size_t hdrnet_model_workspace_bytes_ragged(const hdrnet_model* model,
+                                                      const hdrnet_image_desc* images, int B,
+                                                      int in_fmt, int out_fmt);
+HDRNET_API int hdrnet_model_run_ragged_px(const hdrnet_model* model,
+                                          const hdrnet_image_desc* images, int B, int in_fmt,
+                                          int out_fmt, const hdrnet_image_desc* lowres,
+                                          int lowres_fmt, void* workspace, size_t workspace_bytes,
+                                          void* stream);
+
 #ifdef __cplusplus
 } /* extern "C" */
 #endif

@@ -57,6 +57,15 @@ SIGNATURES = {
     "hdrnet_guide_nn_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong, _c_int]),
     "hdrnet_guide_nn_grad_f32": (_c_int, [_vp] * 3 + [ctypes.c_longlong] + [_vp] * 3
                                  + [ctypes.c_float, _c_int, _vp, _vp, _vp, ctypes.c_size_t, _vp]),
+    # coefficient-network batch norm in training mode: (z, N, C, moments, ws, bytes, stream);
+    # (z, N, C, moments, beta, y, moving_mean, moving_var, stream);
+    # (z, dy, N, C, moments, beta, sums, dbeta, ws, bytes, stream); (z, dy, N, C, moments, beta, sums, dz, stream)
+    "hdrnet_bn_stats_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong, _c_int]),
+    "hdrnet_bn_stats_f32": (_c_int, [_vp, ctypes.c_longlong, _c_int, _vp, _vp, ctypes.c_size_t, _vp]),
+    "hdrnet_bn_relu_f32": (_c_int, [_vp, ctypes.c_longlong, _c_int] + [_vp] * 6),
+    "hdrnet_bn_relu_grad_sums_f32": (_c_int, [_vp, _vp, ctypes.c_longlong, _c_int] + [_vp] * 5
+                                     + [ctypes.c_size_t, _vp]),
+    "hdrnet_bn_relu_grad_f32": (_c_int, [_vp, _vp, ctypes.c_longlong, _c_int] + [_vp] * 5),
     "hdrnet_slice_apply_curves_f32": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 5 + [ctypes.c_float, _vp]),
     "hdrnet_slice_apply_nn_f32": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 3 + [ctypes.c_float, _c_int, _vp]),
     "hdrnet_slice_apply_curves_f32_ws": (_c_int, [_vp] * 4 + [_c_int] * 6 + [_vp] * 5
@@ -70,6 +79,7 @@ SIGNATURES = {
                                     + [_vp] * 3 + [ctypes.c_float, _c_int, _vp, ctypes.c_size_t, _vp]),
     "hdrnet_lowres_nearest_f32": (_c_int, [_vp, _c_int, _vp] + [_c_int] * 5 + [_vp]),
     "hdrnet_conv2d_nhwc_f32": (_c_int, [_vp] * 4 + [_c_int] * 8 + [_vp]),
+    "hdrnet_conv2d_nhwc_fp32_f32": (_c_int, [_vp] * 4 + [_c_int] * 8 + [_vp]),
     "hdrnet_conv2d_tc_packed_bytes": (ctypes.c_size_t, [_c_int] * 3),
     "hdrnet_conv2d_tc_pack_f32": (_c_int, [_vp, _vp] + [_c_int] * 3 + [_vp]),
     "hdrnet_conv2d_nhwc_tc_f32": (_c_int, [_vp] * 4 + [_c_int] * 8 + [_vp]),

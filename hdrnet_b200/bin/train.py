@@ -6,6 +6,7 @@ arguments, flags and defaults (train.py:188-244):
         [--learning_rate 1e-4] [--batch_size 16] [--[no]fliplr|flipud|rotate|random_crop]
         [--model_name HDRNetCurves] [--net_input_size 256] [--output_resolution 512 512] ...
         [--max_steps N] [--seed S] [--[no]train_guide] [--[no]guide_batch_stats]
+        [--[no]coefficient_batch_stats]
 
 ``data_dir`` holds ``filelist.txt`` and the ``input/`` and ``output/`` folders (or is that
 ``filelist.txt``); hdrnet_b200/data_pipeline.py decodes the pairs once and builds each batch in one
@@ -57,7 +58,15 @@ levels' moving averages get no Adam slots, go into every checkpoint and are rest
 evaluation and ``bin/run.py`` run the guide-fused inference form on them.  The pyramid without both
 flags would train through its inference form, which is not differentiated, so it is refused.
 
-Training-mode batch norm in the coefficient network is not implemented, so ``--batch_norm``, the
+``--batch_norm --coefficient_batch_stats`` trains the coefficient network's batch norm as the
+reference's ``--batch_norm`` does (train.py:92-115): each step runs ``inference(..., is_training=True)``
+with the batch-norm layers normalised by the batch's statistics (the whole batch's under a process
+group) and their ``moving_mean`` / ``moving_variance`` moved once per step, on the device, with no host
+synchronisation; each ``BatchNorm/beta`` is trained with Adam, the moving averages get no Adam slots but
+go into every checkpoint and are restored on resume.  The flag is not a model parameter and is not
+written to ``params.json``.  It needs ``--batch_norm`` (``ValueError``), and with
+``HDRNetPointwiseNNGuide`` and ``HDRNetGaussianPyrNN`` also ``--guide_batch_stats`` (``ValueError``): the
+reference runs every batch norm of the model in training mode.  ``--batch_norm`` without it, the
 pyramid without ``--train_guide --guide_batch_stats``, and ``--train_guide`` with
 ``HDRNetPointwiseNNGuide`` without ``--guide_batch_stats`` are refused before any data is read,
 with the models' own ``NotImplementedError``.
@@ -149,6 +158,10 @@ def build_parser() -> argparse.ArgumentParser:
                                 "moving averages updated), as the reference does (HDRNetPointwiseNNGuide and "
                                 "HDRNetGaussianPyrNN).")
     train_grp.add_argument("--noguide_batch_stats", dest="guide_batch_stats", action="store_false")
+    train_grp.add_argument("--coefficient_batch_stats", dest="coefficient_batch_stats", action="store_true",
+                           help="run the coefficient network's batch norm (--batch_norm) in training mode (batch "
+                                "statistics, moving averages updated) and train its betas, as the reference does.")
+    train_grp.add_argument("--nocoefficient_batch_stats", dest="coefficient_batch_stats", action="store_false")
 
     debug_grp = parser.add_argument_group("debug and profiling")
     debug_grp.add_argument("--profiling", dest="profiling", action="store_true", help="accepted for compatibility; ignored.")
@@ -182,7 +195,7 @@ def build_parser() -> argparse.ArgumentParser:
     model_grp.add_argument("--spatial_bin", default=16, type=int, help="Size of the spatial BGU bins (pixels).")
 
     parser.set_defaults(profiling=False, flipud=False, fliplr=False, rotate=False, random_crop=True, batch_norm=False,
-                        train_guide=False, guide_batch_stats=False)
+                        train_guide=False, guide_batch_stats=False, coefficient_batch_stats=False)
     parser.model_group = model_grp
     return parser
 
@@ -195,14 +208,22 @@ def model_params(parser, args) -> dict:
 PYRAMID_FLAGS = "--train_guide --guide_batch_stats"
 
 
-def refuse_untrainable(params, train_guide=False, guide_batch_stats=False) -> None:
+def refuse_untrainable(params, train_guide=False, guide_batch_stats=False, coefficient_batch_stats=False) -> None:
     """NotImplementedError, with the models' own text, for what cannot be trained: the pyramid model
-    other than with ``train_guide`` and ``guide_batch_stats`` together, training-mode batch norm in
-    the coefficient network and (with ``train_guide``) the pointwise-NN guide without
+    other than with ``train_guide`` and ``guide_batch_stats`` together, the coefficient network's batch
+    norm without ``coefficient_batch_stats`` and (with ``train_guide``) the pointwise-NN guide without
     ``guide_batch_stats``.  Asks the models themselves, on the CPU, with a stand-in variable that
     requires grad (they refuse before any device work).  ValueError for ``guide_batch_stats`` on
-    ``HDRNetCurves``, whose guide has no batch norm."""
+    ``HDRNetCurves``, whose guide has no batch norm, for ``coefficient_batch_stats`` without
+    ``batch_norm``, and for ``coefficient_batch_stats`` on the models with a batch-normed guide without
+    ``guide_batch_stats`` (the reference runs every batch norm of the model in training mode)."""
     S = int(params["net_input_size"])
+    if coefficient_batch_stats and not params["batch_norm"]:
+        raise ValueError("--coefficient_batch_stats runs the coefficient network's batch norm in training mode; "
+                         "it needs --batch_norm")
+    if coefficient_batch_stats and params["model_name"] != "HDRNetCurves" and not guide_batch_stats:
+        raise ValueError(f"--coefficient_batch_stats with {params['model_name']} needs --guide_batch_stats: the "
+                         "reference runs every batch norm of the model, the guide's included, in training mode")
     if params["model_name"] == "HDRNetGaussianPyrNN" and not (train_guide and guide_batch_stats):
         # the pyramid trains only as the reference's recipes train it: all three guides, in training mode
         probe = {COEFFS + "splat/conv1/weights": torch.zeros(1, requires_grad=True)}
@@ -212,10 +233,13 @@ def refuse_untrainable(params, train_guide=False, guide_batch_stats=False) -> No
         except NotImplementedError as e:
             raise NotImplementedError(f"{e}; {PYRAMID_FLAGS} trains the pyramid: its three guides, in "
                                       "training mode") from None
-    if params["batch_norm"]:
+    if params["batch_norm"] and not coefficient_batch_stats:
         probe = {f"{scope}/BatchNorm/beta": torch.zeros(1, requires_grad=True)
                  for scope, use_bn, _ in models._coefficient_specs(params) if use_bn}
-        getattr(models, params["model_name"])._coefficients(torch.zeros(1, S, S, 3), dict(params, weights=probe))
+        try:
+            getattr(models, params["model_name"])._coefficients(torch.zeros(1, S, S, 3), dict(params, weights=probe))
+        except NotImplementedError as e:
+            raise NotImplementedError(f"{e}; --coefficient_batch_stats runs it in training mode and trains it") from None
     if guide_batch_stats and params["model_name"] == "HDRNetCurves":
         raise ValueError("--guide_batch_stats runs the pointwise-NN guide's batch norm in training mode; "
                          "HDRNetCurves' guide has no batch norm")
@@ -327,10 +351,16 @@ class Trainer:
         self.p = dict(params, weights=self.weights)
         if args.train_guide:
             self.p["guide_grad"] = True
-        self.is_training = bool(getattr(args, "guide_batch_stats", False))
-        if self.is_training:
+        coefficient_batch_stats = bool(getattr(args, "coefficient_batch_stats", False))
+        if coefficient_batch_stats:
+            self.p["coefficient_batch_stats"] = True
+        self.is_training = bool(getattr(args, "guide_batch_stats", False)) or coefficient_batch_stats
+        if getattr(args, "guide_batch_stats", False):
             log.info("%s: the guide's batch norm runs in training mode (batch statistics; moving averages "
                      "updated each step)", params["model_name"])
+        if coefficient_batch_stats:
+            log.info("%s: the coefficient network's batch norm runs in training mode (batch statistics; moving "
+                     "averages updated each step)", params["model_name"])
 
     # ---- checkpoints ---------------------------------------------------------------------------
     def _resume(self):
@@ -471,7 +501,8 @@ def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
     params = model_params(parser, args)
-    refuse_untrainable(params, args.train_guide, args.guide_batch_stats)     # before any data is read
+    refuse_untrainable(params, args.train_guide, args.guide_batch_stats,      # before any data is read
+                       args.coefficient_batch_stats)
     world = parallel.world_size() if dist.is_initialized() else int(os.environ.get("WORLD_SIZE", "1"))
     data_pipeline.check_shard((0, world), args.batch_size)
     prefix = checkpoint.latest_checkpoint(args.checkpoint_dir)

@@ -839,6 +839,8 @@ static bool patch_two_groups(long long ctas1, int Cout, int K, int sms) {
   return ctas1 > sms && Cout % 8 == 0 && patch_smem_bytes(K, 2) <= 200 * 1024;
 }
 
+static int conv_dispatch_cuda_cores(const ConvArgs& a, bool pdl, cudaStream_t stream);
+
 static int conv_dispatch(const ConvArgs& a, bool pdl, cudaStream_t stream) {
   if (a.B == 0) return HDRNET_OK;
   {  // Tensor-core path (conv_wgmma.cu).  Each 128-pixel tile runs a fixed-latency chunk loop,
@@ -851,6 +853,11 @@ static int conv_dispatch(const ConvArgs& a, bool pdl, cudaStream_t stream) {
       if (rc != HDRNET_E_UNSUPPORTED) return rc;
     }
   }
+  return conv_dispatch_cuda_cores(a, pdl, stream);
+}
+
+// The CUDA-core forms alone (float32 FMAs, round to nearest), for every shape.
+static int conv_dispatch_cuda_cores(const ConvArgs& a, bool pdl, cudaStream_t stream) {
   const long long total_px = static_cast<long long>(a.B) * a.OH * a.OW;
   const int sms = device_sms();
   const long long big_ctas = ((total_px + 63) / 64) * ((a.Cout + 31) / 32);
@@ -901,6 +908,15 @@ int hdrnet_conv2d_nhwc_f32(const float* in, const float* w, const float* bias, f
   ConvArgs a;
   const int rc = conv_fill(&a, in, w, bias, out, B, H, W, Cin, Cout, k, stride, relu);
   return rc ? rc : conv_dispatch(a, false, static_cast<cudaStream_t>(stream));
+}
+
+int hdrnet_conv2d_nhwc_fp32_f32(const float* in, const float* w, const float* bias, float* out, int B,
+                                int H, int W, int Cin, int Cout, int k, int stride, int relu,
+                                void* stream) {
+  ConvArgs a;
+  const int rc = conv_fill(&a, in, w, bias, out, B, H, W, Cin, Cout, k, stride, relu);
+  if (rc || a.B == 0) return rc;
+  return conv_dispatch_cuda_cores(a, false, static_cast<cudaStream_t>(stream));
 }
 
 int hdrnet_fc_f32(const float* in, const float* w, const float* bias, float* out, int B, int I,

@@ -40,7 +40,11 @@ level with its own batch statistics and moves that level's moving averages, and 
 coefficient network and, with ``params['guide_grad']``, every level's guide and ``fullres_input``,
 through ``_ResizeFn``, whose backward is the VJP of the align-corners resize (``csrc/resize.cu``); its
 inference form is not differentiated.  Batch-norm layers of the coefficient network are not
-differentiated: asking for their gradient raises ``NotImplementedError``.
+differentiated in their folded inference form: asking for their gradient raises
+``NotImplementedError``.  With ``params['coefficient_batch_stats']`` (and ``batch_norm``),
+``inference(..., is_training=True)`` runs them in training mode (``_coefficients_training``, the kernels
+of ``csrc/bn_train.cu``): batch statistics, moving averages moved in place, and gradients for their
+``weights`` and ``BatchNorm/beta``.
 
 Execution (all hand-written sm_90a kernels through the C-ABI, no torch math on the path):
   coefficients  4 splat convs, 2 global convs + 3 FCs, 2 local convs (conv2d / fc kernels),
@@ -559,7 +563,9 @@ def pack_conv_weights(w: torch.Tensor):
 PACKED_CONV_MIN_TILES = 64
 
 
-def _conv(x: torch.Tensor, wb, stride=1, relu=True) -> torch.Tensor:
+def _conv(x: torch.Tensor, wb, stride=1, relu=True, tensor_cores=True) -> torch.Tensor:
+    """One conv layer.  `tensor_cores=False` runs the CUDA-core forms alone
+    (hdrnet_conv2d_nhwc_fp32_f32, float32 rounded to nearest) at every size."""
     w, b = wb[0], wb[1]
     packed = wb[2] if len(wb) > 2 else None
     B, H, W, cin = x.shape
@@ -569,6 +575,12 @@ def _conv(x: torch.Tensor, wb, stride=1, relu=True) -> torch.Tensor:
     oh, ow = -(-H // stride), -(-W // stride)
     out = torch.empty((B, oh, ow, cout), dtype=torch.float32, device=x.device)
     lib = _lib.load()
+    if not tensor_cores:
+        rc = lib.hdrnet_conv2d_nhwc_fp32_f32(x.data_ptr(), w.data_ptr(), 0 if b is None else b.data_ptr(),
+                                             out.data_ptr(), B, H, W, cin, cout, k, stride, int(relu),
+                                             torch.cuda.current_stream(x.device).cuda_stream)
+        _lib.check(rc, "conv2d (CUDA cores)")
+        return out
     if packed is not None and (B * oh * ow + 127) // 128 >= PACKED_CONV_MIN_TILES:
         rc = lib.hdrnet_conv2d_nhwc_tc_f32(x.data_ptr(), packed.data_ptr(),
                                            0 if b is None else b.data_ptr(), out.data_ptr(), B, H,
@@ -617,15 +629,15 @@ class _ConvFn(torch.autograd.Function):
     up), backward hdrnet_conv2d_grad_f32."""
 
     @staticmethod
-    def run(x, w, b, stride, relu, packed=None):
+    def run(x, w, b, stride, relu, packed=None, tensor_cores=True):
         b = None if b is None else b.contiguous()
-        return _conv(x.contiguous(), (w.contiguous(), b, packed), stride=stride, relu=relu)
+        return _conv(x.contiguous(), (w.contiguous(), b, packed), stride=stride, relu=relu, tensor_cores=tensor_cores)
 
     @staticmethod
-    def forward(ctx, x, w, b, stride, relu, packed=None):
+    def forward(ctx, x, w, b, stride, relu, packed=None, tensor_cores=True):
         x, w = x.contiguous(), w.contiguous()
         with torch.cuda.device(x.device):
-            out = _ConvFn.run(x, w, b, stride, relu, packed)
+            out = _ConvFn.run(x, w, b, stride, relu, packed, tensor_cores)
         ctx.save_for_backward(x, w, out)
         ctx.stride, ctx.relu, ctx.has_bias = stride, bool(relu), b is not None
         return out
@@ -650,7 +662,7 @@ class _ConvFn(torch.autograd.Function):
                 B, H, W, cin, cout, k, ctx.stride, int(ctx.relu), _ptr(ws),
                 0 if ws is None else ws.numel() * 4, _stream(x.device))
         _lib.check(rc, "conv2d VJP")
-        return dx, dw, db, None, None, None
+        return dx, dw, db, None, None, None, None
 
 
 class _FcFn(torch.autograd.Function):
@@ -851,11 +863,11 @@ def _update_moving_averages(moving, stats: _BatchStats) -> None:
             v.sub_((v - b) * (1.0 - BN_DECAY))
 
 
-def _moving_averages(wts, scope=GUIDE):
-    """The moving averages of the NN guide under `scope`, which training mode updates in place:
-    float32 tensors that do not require grad (TF does not train them)."""
+def _moving_averages(wts, scope=GUIDE, names=_NN_MOVING):
+    """The moving averages of the NN guide under `scope` (or `names` under it), which training mode
+    updates in place: float32 tensors that do not require grad (TF does not train them)."""
     out = []
-    for n in _NN_MOVING:
+    for n in names:
         key = f"{scope}/{n}"
         v = wts.get(key) if isinstance(wts, dict) else None
         if not isinstance(v, torch.Tensor) or v.dtype != torch.float32:
@@ -866,6 +878,86 @@ def _moving_averages(wts, scope=GUIDE):
                              "updates them in place")
         out.append(v)
     return out
+
+
+# ---- the coefficient network's batch norm in training mode (csrc/bn_train.cu) -------------------
+_BN_MOVING = ("BatchNorm/moving_mean", "BatchNorm/moving_variance")
+
+
+def _coefficient_batch_stats(params) -> bool:
+    """Whether the coefficient network's batch-norm layers run in training mode when is_training is
+    set: params['coefficient_batch_stats'] truthy with params['batch_norm'].  The key without
+    batch_norm is a ValueError (there is no such layer to run)."""
+    if not (isinstance(params, dict) and params.get("coefficient_batch_stats")):
+        return False
+    if not params.get("batch_norm"):
+        raise ValueError("params['coefficient_batch_stats'] runs the coefficient network's batch-norm layers in "
+                         "training mode; params['batch_norm'] is not set, so it has none")
+    return True
+
+
+def _bn_relu(z: torch.Tensor, beta: torch.Tensor, moving) -> tuple:
+    """One batch-norm layer in training mode over z [..., C] (the conv or fc output without bias or
+    relu, contiguous): (y, moments).  moments [3, C] float64 (count, mean, M2) are those of the whole
+    batch, merged over the ranks under a process group (parallel.bn_moments_over_ranks); the moving
+    averages `moving` (mean, variance) move toward them in place.  No host synchronisation."""
+    lib = _lib.load()
+    C = z.shape[-1]
+    N = z.numel() // C
+    moments = torch.empty((3, C), dtype=torch.float64, device=z.device)
+    ws = _workspace(z.device, lib.hdrnet_bn_stats_workspace_bytes(N, C))
+    rc = lib.hdrnet_bn_stats_f32(z.data_ptr(), N, C, moments.data_ptr(), ws.data_ptr(), ws.numel() * 4,
+                                 _stream(z.device))
+    _lib.check(rc, "batch-norm statistics")
+    moments = parallel.bn_moments_over_ranks(moments)
+    y = torch.empty_like(z)
+    rc = lib.hdrnet_bn_relu_f32(z.data_ptr(), N, C, moments.data_ptr(), beta.data_ptr(), y.data_ptr(),
+                                moving[0].data_ptr(), moving[1].data_ptr(), _stream(z.device))
+    _lib.check(rc, "batch norm + relu")
+    return y, moments
+
+
+class _BatchNormReluFn(torch.autograd.Function):
+    """relu(batch_norm(z) + beta) in training mode over z and beta (hdrnet/layers.py:47-54,
+    center=True, scale=False); `moving` is the pair of moving averages it updates, not
+    differentiated.  Backward: hdrnet_bn_relu_grad_sums_f32, the sums merged over the ranks
+    (parallel.bn_sums_over_ranks), then hdrnet_bn_relu_grad_f32.  d beta is this rank's own sum, its
+    share of the whole batch's."""
+
+    @staticmethod
+    def run(z, beta, moving):
+        return _bn_relu(z.contiguous(), beta.contiguous(), moving)[0]
+
+    @staticmethod
+    def forward(ctx, z, beta, moving):
+        z, beta = z.contiguous(), beta.contiguous()
+        with torch.cuda.device(z.device):
+            y, moments = _bn_relu(z, beta, moving)
+        ctx.save_for_backward(z, beta, moments)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        z, beta, moments = ctx.saved_tensors
+        dy = dy.contiguous()
+        C = z.shape[-1]
+        N = z.numel() // C
+        lib = _lib.load()
+        dbeta = torch.empty(C, dtype=torch.float32, device=z.device) if ctx.needs_input_grad[1] else None
+        dz = torch.empty_like(z) if ctx.needs_input_grad[0] else None
+        sums = torch.empty((2, C), dtype=torch.float64, device=z.device)
+        with torch.cuda.device(z.device):
+            ws = _workspace(z.device, lib.hdrnet_bn_stats_workspace_bytes(N, C))
+            rc = lib.hdrnet_bn_relu_grad_sums_f32(z.data_ptr(), dy.data_ptr(), N, C, moments.data_ptr(),
+                                                  beta.data_ptr(), sums.data_ptr(), _ptr(dbeta), ws.data_ptr(),
+                                                  ws.numel() * 4, _stream(z.device))
+            _lib.check(rc, "batch-norm VJP sums")
+            sums = parallel.bn_sums_over_ranks(sums)    # every rank joins, whatever it needs
+            if dz is not None:
+                rc = lib.hdrnet_bn_relu_grad_f32(z.data_ptr(), dy.data_ptr(), N, C, moments.data_ptr(),
+                                                 beta.data_ptr(), sums.data_ptr(), dz.data_ptr(), _stream(z.device))
+                _lib.check(rc, "batch-norm VJP")
+        return dz, dbeta, None
 
 
 class _NNGuideFn(torch.autograd.Function):
@@ -914,11 +1006,13 @@ def _trainable_keys(wts, prefix: str):
 
 
 def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None, nn_guide=False,
-                      is_training=False) -> None:
+                      is_training=False, bn_training=False) -> None:
     """NotImplementedError for every gradient this package does not compute (checked before any
     device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN's inference form).
     The curves guide's variables and fullres_input are differentiated only with params['guide_grad'], the
-    pointwise-NN guide's only with params['guide_grad'] and `is_training` (training-mode batch norm)."""
+    pointwise-NN guide's only with params['guide_grad'] and `is_training` (training-mode batch norm).
+    `bn_training`: the coefficient network's batch-norm layers run in training mode
+    (_coefficient_batch_stats), so their variables may require grad."""
     if not torch.is_grad_enabled() or wts is None:
         return
     if what is not None:
@@ -946,7 +1040,8 @@ def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=N
     if _requires_grad(fullres_input) and not guide_grad:
         raise NotImplementedError("gradients for fullres_input are not implemented: they need the guide's "
                                   "backward; pass it with requires_grad=False" + ("" if nn_guide else hint))
-    _refuse_batch_norm(wts, params)
+    if not bn_training:
+        _refuse_batch_norm(wts, params)
 
 
 def _refuse_batch_norm(wts, params) -> None:
@@ -990,15 +1085,21 @@ class HDRNetCurves(object):
         hdrnet_ops.bilateral_slice_apply, whose VJP carries the gradient back to the grid.  The guide
         is a constant there unless params['guide_grad'] is truthy and a curves-guide variable or
         fullres_input requires grad: then it is _CurvesGuideFn, whose VJP takes the slice-apply's
-        guide gradient to the guide variables and adds its input gradient to the slice-apply's."""
-        if is_training:
+        guide gradient to the guide variables and adds its input gradient to the slice-apply's.
+
+        ``is_training=True`` needs params['coefficient_batch_stats'] with params['batch_norm'] (else
+        NotImplementedError): the coefficient network's batch-norm layers then normalise with the
+        batch's statistics and move their moving averages, as _coefficients(..., is_training=True)."""
+        bn_training = _coefficient_batch_stats(params)
+        if is_training and not bn_training:
             raise NotImplementedError("hdrnet_b200 implements the inference path only")
         wts = _weights_or_none(params)
-        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=bool(cls._nn_guide))
+        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=bool(cls._nn_guide),
+                          bn_training=bool(is_training))
         fullres_input = _check_input(fullres_input, "fullres_input")
         coeffs = cls._coefficients(lowres_input, params, is_training)
         if coeffs.requires_grad or (not cls._nn_guide and _guide_grad(wts, params, fullres_input, _CURVES_VARS)):
-            return cls._output(fullres_input, cls._guide(fullres_input, params), coeffs)
+            return cls._output(fullres_input, cls._guide(fullres_input, params, is_training), coeffs)
         return cls._fullres(coeffs, fullres_input, params, torch.float32)
 
     @classmethod
@@ -1072,9 +1173,14 @@ class HDRNetCurves(object):
 
     @classmethod
     def _coefficients(cls, input_tensor, params, is_training=False):
-        """models.py:62-142 -> [B, gh, gw, gd, n_out, n_in]."""
+        """models.py:62-142 -> [B, gh, gw, gd, n_out, n_in].  ``is_training=True`` runs the batch-norm
+        layers in training mode (_coefficients_training) when _coefficient_batch_stats says so, and
+        raises NotImplementedError otherwise."""
         if is_training:
-            raise NotImplementedError("hdrnet_b200 implements the inference path only")
+            if not _coefficient_batch_stats(params):
+                raise NotImplementedError("hdrnet_b200 implements the inference path only")
+            return cls._coefficients_training(input_tensor, params)
+        _coefficient_batch_stats(params)
         _refuse_batch_norm(_weights_or_none(params), params)
         x = _check_input(input_tensor, "lowres_input")
         prep = _prepare(_resolve_weights(params), params, x.device, cls._nn_guide)
@@ -1089,16 +1195,33 @@ class HDRNetCurves(object):
         return cls._coefficients_layers(x, prep.layers, params["luma_bins"], n_ds, grad)
 
     @classmethod
-    def _coefficients_layers(cls, x, L, gd, n_ds, grad):
+    def _coefficients_layers(cls, x, L, gd, n_ds, grad, bn=None):
         """Layer by layer over the prepared weights: with `grad` every layer an autograd Function
-        (backward through csrc/cnn_grad.cu), else only its forward (`run`)."""
-        conv_fn, fc_fn, fuse_fn = (f.apply if grad else f.run for f in (_ConvFn, _FcFn, _FusePredictFn))
+        (backward through csrc/cnn_grad.cu), else only its forward (`run`).  `bn` maps the scope of
+        each layer that runs batch norm in training mode to its (beta, moving averages): that layer
+        runs without bias or relu, then _BatchNormReluFn, and every conv of the network then runs on the
+        CUDA cores (float32 rounded to nearest): batch norm divides a conv's rounding error by the
+        channel's spread, and the 3xTF32 tensor-core form's error, about 1e-6 of a product, would
+        reach the gradients at 1e-3 to 1e-2 of their range (DESIGN.md row f-14)."""
+        conv_fn, fc_fn, fuse_fn, bn_fn = (f.apply if grad else f.run
+                                          for f in (_ConvFn, _FcFn, _FusePredictFn, _BatchNormReluFn))
         p = "inference/coefficients"
         bs = x.shape[0]
+        bn = bn or {}
+
+        tc = not bn
 
         def conv(x, scope, stride, relu=True):
             w, b, packed = L[f"{p}/{scope}"]
-            return conv_fn(x, w, b, stride, relu, packed)
+            if f"{p}/{scope}" in bn:
+                return bn_fn(conv_fn(x, w, None, stride, False, packed, tc), *bn[f"{p}/{scope}"])
+            return conv_fn(x, w, b, stride, relu, packed, tc)
+
+        def fc(x, scope, relu=True):
+            w, b = L[f"{p}/{scope}"][:2]
+            if f"{p}/{scope}" in bn:
+                return bn_fn(fc_fn(x, w, None, False), *bn[f"{p}/{scope}"])
+            return fc_fn(x, w, b, relu)
 
         with torch.cuda.device(x.device):
             for i in range(n_ds):                                   # splat, :69-82
@@ -1107,14 +1230,48 @@ class HDRNetCurves(object):
             g = conv(splat, "global/conv1", 2)                      # global, :86-105
             g = conv(g, "global/conv2", 2)
             g = g.reshape(bs, -1)                                   # NHWC flatten, :94-95
-            g = fc_fn(g, *L[f"{p}/global/fc1"][:2], True)
-            g = fc_fn(g, *L[f"{p}/global/fc2"][:2], True)
-            g = fc_fn(g, *L[f"{p}/global/fc3"][:2], False)
+            g = fc(g, "global/fc1")
+            g = fc(g, "global/fc2")
+            g = fc(g, "global/fc3", False)
             loc = conv(splat, "local/conv1", 1)                     # local, :109-118
             loc = conv(loc, "local/conv2", 1, relu=False)
             wp, bp = L[f"{p}/prediction/conv1"][:2]                 # HWIO [1, 1, C, O] -> [C, O]
             # fusion + prediction + unroll, :122-139
             return fuse_fn(loc, g, wp.reshape(wp.shape[-2:]), bp, gd, cls.n_out(), cls.n_in())
+
+    @classmethod
+    def _coefficients_training(cls, input_tensor, params):
+        """The coefficient network with its batch-norm layers in training mode (hdrnet/layers.py:47-54,
+        is_training=True): each normalises with the batch's statistics (the whole batch's under a
+        process group) and moves its ``BatchNorm/moving_mean`` and ``moving_variance`` (float32 tensors
+        on the input's device that do not require grad) in place, once per call.  Layer by layer on
+        the raw variables, nothing folded and no host synchronisation; ``weights``, ``BatchNorm/beta``,
+        the other layers' variables and ``lowres_input`` are differentiated where they require grad."""
+        wts = _resolve_weights(params)
+        specs = _coefficient_specs(params)
+        moving = {scope: _moving_averages(wts, scope, _BN_MOVING) for scope, use_bn, _ in specs if use_bn}
+        x = _check_input(input_tensor, "lowres_input")
+        if x.shape[0] == 0:
+            raise ValueError("lowres_input is empty: batch statistics need at least one image")
+        for scope, pair in moving.items():
+            for name, v in zip(_BN_MOVING, pair):
+                if v.device != x.device or not v.is_contiguous():
+                    raise ValueError(f"{scope}/{name} must be a contiguous tensor on {x.device}: is_training=True "
+                                     "updates it in place there")
+        dev = x.device
+        layers_, bn = {}, {}
+        with torch.cuda.device(dev):
+            for scope, use_bn, use_bias in specs:
+                w = _device_var(wts[scope + "/weights"], dev)
+                b = _device_var(wts[scope + "/biases"], dev) if use_bias and not use_bn else None
+                layers_[scope] = (w, b, None)      # the convs run on the CUDA cores (_coefficients_layers)
+                if use_bn:
+                    bn[scope] = (_device_var(wts[scope + "/BatchNorm/beta"], dev), moving[scope])
+        grad = torch.is_grad_enabled() and (x.requires_grad or any(
+            _requires_grad(t) for wb in layers_.values() for t in wb[:2]) or
+            any(_requires_grad(beta) for beta, _ in bn.values()))
+        n_ds = int(np.log2(params["net_input_size"] / params["spatial_bin"]))
+        return cls._coefficients_layers(x, layers_, params["luma_bins"], n_ds, grad, bn)
 
     @classmethod
     def _coefficients_chain(cls, x, prep, params):
@@ -1155,6 +1312,8 @@ class HDRNetCurves(object):
         if _guide_grad(wts, params, x, _CURVES_VARS):
             with torch.cuda.device(x.device):
                 return _CurvesGuideFn.apply(x, *[wts["inference/guide/" + n] for n in _CURVES_VARS])
+        if is_training:    # the coefficient layers are not prepared (folded, packed) for the guide alone
+            return _CurvesGuide.from_weights(wts).run(x)
         return _prepare(wts, params, x.device, False).guides[0].run(x)
 
     @classmethod
@@ -1184,14 +1343,17 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
         if not is_training:
             return super().inference(lowres_input, fullres_input, params)
         wts = _resolve_weights(params)
-        if params.get("batch_norm"):
+        bn_training = _coefficient_batch_stats(params)
+        if params.get("batch_norm") and not bn_training:
             raise NotImplementedError(
                 "training-mode batch norm in the coefficient network (params['batch_norm']) is not "
-                "implemented: only the guide's conv1 batch norm runs in training mode")
+                "implemented: only the guide's conv1 batch norm runs in training mode; "
+                "params['coefficient_batch_stats'] runs the coefficient network's in training mode too")
         _moving_averages(wts)
-        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True)
+        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True,
+                          bn_training=bn_training)
         fullres_input = _check_input(fullres_input, "fullres_input")
-        coeffs = cls._coefficients(lowres_input, params)
+        coeffs = cls._coefficients(lowres_input, params, bn_training)
         return cls._output(fullres_input, cls._guide(fullres_input, params, is_training=True), coeffs)
 
     @classmethod
@@ -1206,7 +1368,8 @@ class HDRNetPointwiseNNGuide(HDRNetCurves):
         if is_training:
             wts = _resolve_weights(params)
             moving = _moving_averages(wts, scope)
-            _refuse_untrained(wts, params, fullres_input=input_tensor, nn_guide=True, is_training=True)
+            _refuse_untrained(wts, params, fullres_input=input_tensor, nn_guide=True, is_training=True,
+                              bn_training=_coefficient_batch_stats(params))
             x = _check_input(input_tensor, "fullres_input")
             if x.numel() == 0:
                 raise ValueError("fullres_input is empty: batch statistics need at least one pixel")
@@ -1325,15 +1488,18 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
         the pyramid, the three levels' guides (level 0 first, on every rank) and the coarse-to-fine
         output through hdrnet_ops' slice-apply."""
         wts = _resolve_weights(params)
-        if params.get("batch_norm"):
+        bn_training = _coefficient_batch_stats(params)
+        if params.get("batch_norm") and not bn_training:
             raise NotImplementedError(
                 "training-mode batch norm in the coefficient network (params['batch_norm']) is not "
-                "implemented: only the guides' conv1 batch norm runs in training mode")
+                "implemented: only the guides' conv1 batch norm runs in training mode; "
+                "params['coefficient_batch_stats'] runs the coefficient network's in training mode too")
         for scope in cls._guide_scopes():
             _moving_averages(wts, scope)
-        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True)
+        _refuse_untrained(wts, params, fullres_input=fullres_input, nn_guide=True, is_training=True,
+                          bn_training=bn_training)
         fullres_input = _check_input(fullres_input, "fullres_input")
-        coeffs = cls._coefficients(lowres_input, params)
+        coeffs = cls._coefficients(lowres_input, params, bn_training)
         with torch.cuda.device(fullres_input.device):
             multiscale = cls._multiscale_input(fullres_input)
             guides = cls._guide(multiscale, params, is_training=True)

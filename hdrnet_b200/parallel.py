@@ -10,7 +10,9 @@ distributed code at all (SURVEY.md section 2b).
 
 Data-parallel training (bin/train.py under torchrun) adds, per step, one all-reduce of the flat
 gradient buffer (all_reduce_mean_) and one of a few scalars (sum_over_ranks); the pointwise-NN guide's
-training-mode batch norm adds one all-gather of the input moments (moments_over_ranks); and each
+training-mode batch norm adds one all-gather of the input moments (moments_over_ranks); the coefficient
+network's, with --coefficient_batch_stats, one all-gather of each batch-norm layer's moments in the
+forward and of its VJP sums in the backward (bn_moments_over_ranks, bn_sums_over_ranks); and each
 checkpoint one all-gather of a digest of the state (check_ranks_agree).
 """
 from __future__ import annotations
@@ -25,7 +27,7 @@ import torch.distributed as dist
 __all__ = ["init_distributed", "shard_batch", "shard_rows", "shard_plan", "slice_apply_sharded",
            "broadcast_weights", "max_over_ranks", "finalize", "bind_to_gpu_numa", "gpu_cpu_affinity",
            "world_size", "all_reduce_mean_", "sum_over_ranks", "merge_moments", "moments_over_ranks",
-           "check_ranks_agree"]
+           "bn_moments_over_ranks", "bn_sums_over_ranks", "check_ranks_agree"]
 
 
 def gpu_cpu_affinity(device_index: int) -> list[int]:
@@ -250,6 +252,46 @@ def moments_over_ranks(moments, npix: int):
         row = row.to(torch.device("cuda", torch.cuda.current_device()))
     rows = _all_gather(row)
     return merge_moments(rows[:, 0], rows[:, 1:]), int(rows[:, 0].sum())
+
+
+def _all_gather_tensor(t: torch.Tensor) -> torch.Tensor:
+    """[world, *t.shape]: every rank's ``t``, in rank order, on ``t``'s device (staged through the host
+    with gloo)."""
+    buf = _staged(t.contiguous())
+    parts = [torch.empty_like(buf) for _ in range(world_size())]
+    dist.all_gather(parts, buf)
+    return torch.stack(parts).to(t.device)
+
+
+def bn_moments_over_ranks(moments: torch.Tensor) -> torch.Tensor:
+    """The batch-norm moments of the whole batch from this rank's ``moments`` [3, C] (float64 count,
+    mean and M2 per channel over its rows, as hdrnet_bn_stats_f32 writes them): one all-gather, then
+    the ranks merged in rank order (Chan et al.) in float64, so every rank gets the same bits.  Without
+    a group: ``moments`` itself, and nothing leaves the device."""
+    if world_size() == 1:
+        return moments
+    parts = _all_gather_tensor(moments)
+    n, mean, m2 = parts[0].unbind(0)
+    for nb, mb, m2b in parts[1:]:
+        nt = n + nb
+        d = mb - mean
+        mean = mean + d * (nb / nt)
+        m2 = m2 + m2b + d * d * (n * nb / nt)
+        n = nt
+    return torch.stack([n, mean, m2])
+
+
+def bn_sums_over_ranks(sums: torch.Tensor) -> torch.Tensor:
+    """The batch-norm VJP sums [2, C] (float64 A and B per channel, hdrnet_bn_relu_grad_sums_f32) of
+    the whole batch: one all-gather, added in rank order, so every rank gets the same bits.  Without a
+    group: ``sums`` itself."""
+    if world_size() == 1:
+        return sums
+    parts = _all_gather_tensor(sums)
+    total = parts[0]
+    for p in parts[1:]:
+        total = total + p
+    return total
 
 
 def check_ranks_agree(arrays, what: str = "the training state") -> None:

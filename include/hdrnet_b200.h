@@ -281,6 +281,55 @@ HDRNET_API int hdrnet_guide_nn_grad_f32(const float* input, const float* dguide,
                                         size_t workspace_bytes, void* stream);
 
 /*
+ * Training-mode batch norm of the coefficient network's layers (hdrnet/layers.py:47-54 with
+ * is_training=True, center=True, scale=False, epsilon 1e-3, decay 0.999).  z is the layer's conv
+ * or fc output WITHOUT bias or relu (hdrnet_conv2d_nhwc_f32 / hdrnet_fc_f32 with bias NULL and
+ * relu 0), an [N, C] row-major float32 view (NHWC flattened; an fc layer has N = B).  Every
+ * pointer is a DEVICE pointer; nothing is read back to the host.  N >= 1 and
+ * 1 <= C <= HDRNET_BN_MAX_CHANNELS (larger: HDRNET_E_UNSUPPORTED).  Float arrays must be 4-byte
+ * and double arrays and workspaces 8-byte aligned (HDRNET_E_BAD_SHAPE otherwise).
+ *
+ * moments [3][C] (float64) holds per channel the row count n, the mean and the sum of squared
+ * deviations M2, so that the moments of several ranks' shards merge exactly (Chan et al.).
+ *
+ * hdrnet_bn_stats_f32: the moments of z over its N rows (n = N).  Per-CTA partials of fixed row
+ * chunks (chosen from N and C alone), each centred on its first row, go to a caller-lent
+ * workspace of hdrnet_bn_stats_workspace_bytes(N, C) bytes (smaller: HDRNET_E_BAD_SHAPE) and are
+ * merged in float64 in a fixed order: no atomics, bitwise reproducible.
+ *
+ * hdrnet_bn_relu_f32: y [N, C] = relu((z - mean) / sqrt(M2 / n + 1e-3) + beta [C]).  When
+ * moving_mean and moving_var [C] are given (both or neither) they move toward the batch's
+ * statistics in place, as TF's moving-average update does without zero-debias:
+ * v -= (1 - 0.999) (v - batch), the variance fed to it Bessel-corrected, M2 / n * n / (n - 1)
+ * (0 for n = 1).
+ *
+ * hdrnet_bn_relu_grad_sums_f32: with dy [N, C] the gradient of y and dyh = dy [y > 0] (TF's
+ * ReluGrad on the y hdrnet_bn_relu_f32 computes), sums [2][C] (float64) receives
+ * A = sum dyh and B = sum dyh (z - mean) s over this call's N rows, and dbeta [C] (optional) A as
+ * float32.  The workspace is that of hdrnet_bn_stats_f32 (hdrnet_bn_stats_workspace_bytes), the
+ * same fixed chunks summed in a fixed order.
+ *
+ * hdrnet_bn_relu_grad_f32: dz [N, C] = s (dyh - A / n - (z - mean) s B / n), with n, A and B
+ * from moments and sums.  Split from the sums so that the sums of several ranks can be added
+ * between the two calls, as their moments are merged before hdrnet_bn_relu_f32.
+ * The workspaces are scratch, undefined after the call.
+ */
+#define HDRNET_BN_MAX_CHANNELS 8192
+HDRNET_API size_t hdrnet_bn_stats_workspace_bytes(long long N, int C);
+HDRNET_API int hdrnet_bn_stats_f32(const float* z, long long N, int C, double* moments,
+                                   void* workspace, size_t workspace_bytes, void* stream);
+HDRNET_API int hdrnet_bn_relu_f32(const float* z, long long N, int C, const double* moments,
+                                  const float* beta, float* y, float* moving_mean,
+                                  float* moving_var, void* stream);
+HDRNET_API int hdrnet_bn_relu_grad_sums_f32(const float* z, const float* dy, long long N, int C,
+                                            const double* moments, const float* beta,
+                                            double* sums, float* dbeta, void* workspace,
+                                            size_t workspace_bytes, void* stream);
+HDRNET_API int hdrnet_bn_relu_grad_f32(const float* z, const float* dy, long long N, int C,
+                                       const double* moments, const float* beta,
+                                       const double* sums, float* dz, void* stream);
+
+/*
  * Model-path forms of slice-apply: the guide is computed per pixel INSIDE the kernel from the
  * full-res RGB (the guide map never touches HBM: 24 B/px instead of 28 B/px + a guide pass).
  * Replaces HDRNetCurves.inference / HDRNetPointwiseNNGuide.inference's `_guide` + `_output`
@@ -330,6 +379,16 @@ HDRNET_API int hdrnet_conv2d_tc_pack_f32(const float* w, float* packed, int k, i
 HDRNET_API int hdrnet_conv2d_nhwc_tc_f32(const float* in, const float* packed_w, const float* bias,
                                          float* out, int B, int H, int W, int Cin, int Cout,
                                          int k, int stride, int relu, void* stream);
+
+/*
+ * conv2d on the CUDA cores alone (float32 FMAs rounded to nearest), at every shape: what
+ * hdrnet_conv2d_nhwc_f32 runs below 96 tiles.  Its tensor-core form from 96 tiles up (3xTF32)
+ * is float32-grade to about 1e-6 of a product; training-mode batch norm divides a conv's error by
+ * the channel's spread, and runs its convs here.
+ */
+HDRNET_API int hdrnet_conv2d_nhwc_fp32_f32(const float* in, const float* w, const float* bias,
+                                           float* out, int B, int H, int W, int Cin, int Cout,
+                                           int k, int stride, int relu, void* stream);
 
 /* fully_connected: out[B,O] = in[B,I] @ w[I,O] + bias (+ReLU). */
 HDRNET_API int hdrnet_fc_f32(const float* in, const float* w, const float* bias, float* out,

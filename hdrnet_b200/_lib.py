@@ -100,6 +100,11 @@ SIGNATURES = {
     "hdrnet_coefficients_f32": (_c_int, [_vp] * 4 + [_c_int, _vp, ctypes.c_size_t] + [_c_int] * 7 + [_vp]),
     # (samples, B, fullres_in, fullres_out, lowres_in, oh, ow, S, stream)
     "hdrnet_train_batch_f32": (_c_int, [_vp, _c_int] + [_vp] * 3 + [_c_int] * 3 + [_vp]),
+    # (samples, B, oh, ow, sigma); (samples, B, fullres_in, fullres_out, lowres_in, oh, ow, S, sigma,
+    # sharpen, ws, bytes, stream)
+    "hdrnet_train_batch_usm_workspace_bytes": (ctypes.c_size_t, [_vp] + [_c_int] * 3 + [ctypes.c_double]),
+    "hdrnet_train_batch_usm_f32": (_c_int, [_vp, _c_int] + [_vp] * 3 + [_c_int] * 3
+                                   + [ctypes.c_double] * 2 + [_vp, ctypes.c_size_t, _vp]),
     "hdrnet_host_ctx_create": (_c_int, [ctypes.POINTER(_vp), ctypes.c_size_t]),
     "hdrnet_host_ctx_destroy": (_c_int, [_vp]),
     "hdrnet_slice_apply_host_f32": (_c_int, [_vp] * 5 + [_c_int] * 9),
@@ -149,6 +154,14 @@ class TrainSample(ctypes.Structure):
     _fields_ = [("input", _vp), ("target", _vp), ("input_fmt", _c_int), ("target_fmt", _c_int),
                 ("H", _c_int), ("W", _c_int), ("fliplr", _c_int), ("flipud", _c_int),
                 ("rot90", _c_int), ("crop_y", _c_int), ("crop_x", _c_int)]
+
+
+class UsmSample(ctypes.Structure):
+    """hdrnet_usm_sample: one sample's descriptor for hdrnet_train_batch_usm_f32 (a window of the
+    full H x W source, and the draw on the full source's rotated extent)."""
+    _fields_ = [("input", _vp), ("input_fmt", _c_int), ("H", _c_int), ("W", _c_int),
+                ("y0", _c_int), ("x0", _c_int), ("h", _c_int), ("w", _c_int),
+                ("fliplr", _c_int), ("flipud", _c_int), ("rot90", _c_int), ("crop_y", _c_int), ("crop_x", _c_int)]
 
 _lock = threading.Lock()
 _lib = None

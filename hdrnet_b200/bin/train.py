@@ -6,7 +6,7 @@ arguments, flags and defaults (train.py:188-244):
         [--learning_rate 1e-4] [--batch_size 16] [--[no]fliplr|flipud|rotate|random_crop]
         [--model_name HDRNetCurves] [--net_input_size 256] [--output_resolution 512 512] ...
         [--max_steps N] [--seed S] [--[no]train_guide] [--[no]guide_batch_stats]
-        [--[no]coefficient_batch_stats]
+        [--[no]coefficient_batch_stats] [--data_pipeline UnsharpMaskDataPipeline --blur_sigma S --sharpen A]
 
 ``data_dir`` holds ``filelist.txt`` and the ``input/`` and ``output/`` folders (or is that
 ``filelist.txt``); hdrnet_b200/data_pipeline.py decodes the pairs once and builds each batch in one
@@ -88,12 +88,25 @@ ranks.  The world size is not a model parameter and is not written to ``params.j
 resumes with any world size, since the batches depend only on ``(seed, step)`` and the global batch.
 Without ``WORLD_SIZE`` (or with 1) no process group is made and no collective runs.
 
+``--data_pipeline UnsharpMaskDataPipeline --blur_sigma S --sharpen A`` trains from input images alone,
+as the reference's ``scripts/usm/*.sh`` recipes do: ``data_dir`` (and ``--eval_data_dir``) needs
+``filelist.txt`` and ``input/`` only, and each target is the unsharp mask
+``clip(x + A (x - G_S * x), 0, 1)`` of its input, computed on the device in source coordinates
+(data_pipeline.UnsharpMaskDataPipeline defines it).  Both flags are required with that pipeline and
+refused with ``ImageFilesDataPipeline``; 0 < S <= 32 and a finite A, else the parser refuses.  The two
+values go into every checkpoint as the scalars ``train/usm_blur_sigma`` and ``train/usm_sharpen``
+(``bin/run.py``, ``freeze_model`` and ``import_checkpoint`` read only ``inference/*``), and a resume
+with other values, or with the other pipeline, is refused before any data is read.
+
 Deliberate differences from the reference:
 
 * ``--max_steps`` (the reference runs until interrupted), ``--seed``, ``--train_guide`` and
   ``--guide_batch_stats`` are added (the reference always trains the guide, in training mode; here
   both are opt-in);
-  ``--data_pipeline`` takes only ``ImageFilesDataPipeline`` (the tfrecord pipelines need TF);
+  ``--data_pipeline`` takes ``ImageFilesDataPipeline`` and ``UnsharpMaskDataPipeline`` (the tfrecord
+  pipelines need TF).  The reference's ``data_pipeline.py`` does not define ``UnsharpMaskDataPipeline``
+  and its parser has no ``--blur_sigma`` or ``--sharpen``, though its ``usm/`` scripts pass them; the
+  pipeline and both flags are this project's definition (data_pipeline.py);
   ``--profiling`` is accepted and ignored.
 * The evaluation reads ``--eval_data_dir``.  The reference builds the eval pipeline but then
   evaluates the training samples (train.py:86 takes ``train_data_pipeline.samples``, and :105
@@ -179,6 +192,11 @@ def build_parser() -> argparse.ArgumentParser:
     data_grp.add_argument("--nofliplr", dest="fliplr", action="store_false")
     data_grp.add_argument("--random_crop", dest="random_crop", action="store_true", help="random crop data augmentation.")
     data_grp.add_argument("--norandom_crop", dest="random_crop", action="store_false")
+    data_grp.add_argument("--blur_sigma", default=None, type=float,
+                          help="UnsharpMaskDataPipeline: standard deviation of the target's Gaussian blur, in source "
+                               "pixels (0 < S <= 32).")
+    data_grp.add_argument("--sharpen", default=None, type=float,
+                          help="UnsharpMaskDataPipeline: the target is clip(x + sharpen * (x - blur(x)), 0, 1).")
 
     model_grp = parser.add_argument_group("model_params")
     model_grp.add_argument("--model_name", default=models.__all__[0], type=str, help="classname of the model to use.",
@@ -203,6 +221,32 @@ def build_parser() -> argparse.ArgumentParser:
 def model_params(parser, args) -> dict:
     """The model_params group, as train.py:250-252 collects it (and params.json stores it)."""
     return {a.dest: getattr(args, a.dest, None) for a in parser.model_group._group_actions}
+
+
+def check_data_flags(parser, args) -> None:
+    """parser.error unless ``--blur_sigma`` and ``--sharpen`` are given exactly with
+    ``--data_pipeline UnsharpMaskDataPipeline``, with values ``data_pipeline.check_usm`` accepts."""
+    given = [f for f in ("blur_sigma", "sharpen") if getattr(args, f, None) is not None]
+    if args.data_pipeline == "UnsharpMaskDataPipeline":
+        if len(given) != 2:
+            parser.error("--data_pipeline UnsharpMaskDataPipeline needs --blur_sigma and --sharpen")
+        try:
+            data_pipeline.check_usm(args.blur_sigma, args.sharpen)
+        except ValueError as e:
+            parser.error(f"--blur_sigma / --sharpen: {e}")
+    elif given:
+        parser.error(f"--{given[0]} sets the unsharp-mask target of --data_pipeline UnsharpMaskDataPipeline; "
+                     f"{args.data_pipeline} reads its targets from output/")
+
+
+def usm_values(args):
+    """``(blur_sigma, sharpen)`` of an UnsharpMaskDataPipeline run, else None."""
+    if getattr(args, "data_pipeline", "ImageFilesDataPipeline") != "UnsharpMaskDataPipeline":
+        return None
+    return float(args.blur_sigma), float(args.sharpen)
+
+
+USM_KEYS = ("train/usm_blur_sigma", "train/usm_sharpen")
 
 
 PYRAMID_FLAGS = "--train_guide --guide_batch_stats"
@@ -252,9 +296,21 @@ def refuse_untrainable(params, train_guide=False, guide_batch_stats=False, coeff
             raise NotImplementedError(f"{e}; --guide_batch_stats runs it in training mode and trains it") from None
 
 
-def refuse_resume_mismatch(saved: dict, train_guide: bool) -> None:
-    """ValueError when a checkpoint to resume was written with the other --[no]train_guide: its guide
-    variables have Adam slots exactly when it trained them."""
+def refuse_resume_mismatch(saved: dict, train_guide: bool, usm=None) -> None:
+    """ValueError when a checkpoint to resume was written with the other --[no]train_guide (its guide
+    variables have Adam slots exactly when it trained them), or with another data pipeline or other
+    unsharp-mask values than ``usm`` (``usm_values``: the checkpoint's ``train/usm_*`` scalars)."""
+    saved_usm = tuple(float(saved[k]) for k in USM_KEYS) if all(k in saved for k in USM_KEYS) else None
+    if usm is None and saved_usm is not None:
+        raise ValueError("the checkpoint to resume was trained with --data_pipeline UnsharpMaskDataPipeline "
+                         f"--blur_sigma {saved_usm[0]:g} --sharpen {saved_usm[1]:g}: resume it with those flags")
+    if usm is not None and saved_usm is None:
+        raise ValueError("the checkpoint to resume was trained on image pairs (ImageFilesDataPipeline): resume it "
+                         "without --data_pipeline UnsharpMaskDataPipeline, or start a new checkpoint_dir")
+    if usm is not None and tuple(float(v) for v in usm) != saved_usm:
+        raise ValueError(f"the checkpoint to resume was trained with --blur_sigma {saved_usm[0]!r} --sharpen "
+                         f"{saved_usm[1]!r}, not {float(usm[0])!r} and {float(usm[1])!r}: resume it with its own "
+                         "values, or start a new checkpoint_dir")
     has_slots = any(k.startswith(GUIDE) and k.endswith(("/Adam", "/Adam_1")) for k in saved)
     if train_guide and not has_slots:
         raise ValueError("the checkpoint to resume was trained with the guide held fixed (no Adam slots for "
@@ -277,10 +333,12 @@ def slot_names(name):
     return name + "/Adam", name + "/Adam_1"
 
 
-def checkpoint_tensors(variables: dict, moments: dict, step: int, ema: dict) -> dict:
+def checkpoint_tensors(variables: dict, moments: dict, step: int, ema: dict, usm=None) -> dict:
     """What a checkpoint holds, as numpy arrays: the variables, Adam's moments ``{name: (m, v)}``
     under TF's slot names, ``global_step`` (int64), TF's ``beta1_power`` / ``beta2_power``
-    accumulators (beta^(step + 1)) and the logged moving averages."""
+    accumulators (beta^(step + 1)), the logged moving averages and, for an UnsharpMaskDataPipeline
+    run, ``usm = (blur_sigma, sharpen)`` as float64 scalars ``train/usm_blur_sigma`` and
+    ``train/usm_sharpen``."""
     t = {k: np.asarray(v) for k, v in variables.items()}
     for k, (m, v) in moments.items():
         sm, sv = slot_names(k)
@@ -290,6 +348,9 @@ def checkpoint_tensors(variables: dict, moments: dict, step: int, ema: dict) -> 
     t["beta2_power"] = np.array(BETA2 ** (step + 1), np.float32)
     for key, val in ema.items():
         t[f"train/{key}_ema"] = np.array(val, np.float64)
+    if usm is not None:
+        for key, val in zip(USM_KEYS, usm):
+            t[key] = np.array(val, np.float64)
     return t
 
 
@@ -338,16 +399,23 @@ class Trainer:
             log.info("%s: training the %d coefficient-network variables; the guide variables (%s*) are held fixed "
                      "at their %s values", params["model_name"], len(self.names), GUIDE,
                      "restored" if self.step else "initial")
-        self.train_data = data_pipeline.ImageFilesDataPipeline(
+        self.usm = usm_values(args)
+        if self.usm is None:
+            pipeline, usm_kw = data_pipeline.ImageFilesDataPipeline, {}
+        else:
+            pipeline = data_pipeline.UnsharpMaskDataPipeline
+            usm_kw = {"blur_sigma": self.usm[0], "sharpen": self.usm[1]}
+            log.info("targets: unsharp masks of the inputs (blur_sigma %g, sharpen %g)", *self.usm)
+        self.train_data = pipeline(
             args.data_dir, batch_size=args.batch_size, output_resolution=args.output_resolution, shuffle=True,
             fliplr=args.fliplr, flipud=args.flipud, rotate=args.rotate, random_crop=args.random_crop,
             params=params, nthreads=args.data_threads, seed=args.seed, device=self.device,
-            shard=(self.rank, self.world))
+            shard=(self.rank, self.world), **usm_kw)
         self.eval_data = None
         if args.eval_data_dir is not None:
-            self.eval_data = data_pipeline.ImageFilesDataPipeline(
+            self.eval_data = pipeline(
                 args.eval_data_dir, batch_size=1, output_resolution=args.output_resolution, shuffle=False,
-                params=params, nthreads=1, device=self.device)
+                params=params, nthreads=1, device=self.device, **usm_kw)
         self.p = dict(params, weights=self.weights)
         if args.train_guide:
             self.p["guide_grad"] = True
@@ -368,7 +436,7 @@ class Trainer:
         if prefix is None:
             return
         saved = checkpoint.read_tf_checkpoint(prefix)
-        refuse_resume_mismatch(saved, self.args.train_guide)
+        refuse_resume_mismatch(saved, self.args.train_guide, usm_values(self.args))
         values, moments, step, ema = restored_state(saved, self.weights, self.names)
         with torch.no_grad():
             for k, v in self.weights.items():
@@ -399,7 +467,8 @@ class Trainer:
                                        f"the variables and Adam moments at step {self.step}")
         if self.rank:
             return prefix
-        checkpoint.write_tf_checkpoint(prefix, checkpoint_tensors(variables, moments, self.step, self.ema))
+        checkpoint.write_tf_checkpoint(prefix, checkpoint_tensors(variables, moments, self.step, self.ema,
+                                                                  usm_values(self.args)))
         with open(os.path.join(self.args.checkpoint_dir, "params.json"), "w") as f:
             json.dump(self.params, f)
         log.info("saved %s", prefix)
@@ -500,6 +569,7 @@ class Trainer:
 def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
+    check_data_flags(parser, args)
     params = model_params(parser, args)
     refuse_untrainable(params, args.train_guide, args.guide_batch_stats,      # before any data is read
                        args.coefficient_batch_stats)
@@ -507,7 +577,7 @@ def main(argv=None):
     data_pipeline.check_shard((0, world), args.batch_size)
     prefix = checkpoint.latest_checkpoint(args.checkpoint_dir)
     if prefix is not None:
-        refuse_resume_mismatch(checkpoint.read_tf_checkpoint(prefix), args.train_guide)
+        refuse_resume_mismatch(checkpoint.read_tf_checkpoint(prefix), args.train_guide, usm_values(args))
     if args.profiling:
         log.warning("--profiling is accepted for compatibility and ignored")
     if not torch.cuda.is_available():

@@ -1,5 +1,6 @@
 """Training data from image pairs, batched on the device: the reference's ``ImageFilesDataPipeline``
-(hdrnet/data_pipeline.py:126-240).
+(hdrnet/data_pipeline.py:126-240); and from input images alone, ``UnsharpMaskDataPipeline``, whose
+targets are unsharp masks of the inputs (this project's definition: its class docstring).
 
 Layout (data_pipeline.py:174-200): ``<data_dir>/filelist.txt`` names one file per line; the pair is
 ``<data_dir>/input/<name>`` and ``<data_dir>/output/<name>``.  ``path`` may be the directory or the
@@ -56,7 +57,7 @@ import torch
 
 from . import _lib
 
-__all__ = ["ImageFilesDataPipeline"]
+__all__ = ["ImageFilesDataPipeline", "UnsharpMaskDataPipeline"]
 
 log = logging.getLogger("data_pipeline")
 
@@ -110,6 +111,22 @@ def load_pairs(path: str, nthreads: int = 1):
     with concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads))) as ex:
         ims = list(ex.map(decode_image, files))
     return names, ims[0::2], ims[1::2], dirname
+
+
+def load_inputs(path: str, nthreads: int = 1):
+    """(names, inputs, data directory): every input named by the file list, decoded; ``output/`` is
+    not read (UnsharpMaskDataPipeline computes its targets)."""
+    dirname, filelist = data_paths(path)
+    names = read_filelist(filelist)
+    with concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads))) as ex:
+        ims = list(ex.map(decode_image, [os.path.join(dirname, "input", n) for n in names]))
+    return names, ims, dirname
+
+
+def check_inputs(names, inputs, dirname, output_resolution, rotate: bool) -> None:
+    """ValueError naming the file when an input is smaller than ``output_resolution`` for a rotation
+    the flags allow: ``check_pairs`` for a pipeline without target images."""
+    check_pairs(names, inputs, inputs, dirname, output_resolution, rotate)
 
 
 def check_pairs(names, inputs, targets, dirname, output_resolution, rotate: bool) -> None:
@@ -303,6 +320,109 @@ def slot_bytes(formats, batch_size: int, output_resolution) -> int:
     return int(batch_size) * widest
 
 
+USM_MAX_SIGMA = 32.0    # radius int(4 * 32 + 0.5) = 128
+
+
+def check_usm(blur_sigma, sharpen):
+    """``(blur_sigma, sharpen)`` as floats; ValueError unless 0 < blur_sigma <= 32 and sharpen is
+    finite."""
+    try:
+        sigma, amount = float(blur_sigma), float(sharpen)
+    except (TypeError, ValueError):
+        raise ValueError(f"blur_sigma {blur_sigma!r} and sharpen {sharpen!r} must be numbers") from None
+    if not 0.0 < sigma <= USM_MAX_SIGMA:
+        raise ValueError(f"blur_sigma must be in (0, {USM_MAX_SIGMA:g}] source pixels, got {blur_sigma!r}")
+    if not np.isfinite(amount):
+        raise ValueError(f"sharpen must be a finite number, got {sharpen!r}")
+    return sigma, amount
+
+
+def usm_radius(blur_sigma) -> int:
+    """The Gaussian's radius in source pixels: scipy.ndimage.gaussian_filter1d's ``int(4.0 * sigma + 0.5)``."""
+    return int(4.0 * float(blur_sigma) + 0.5)
+
+
+def grown_window(H: int, W: int, draw: Draw, oh: int, ow: int, radius: int):
+    """``(y0, x0, h, w)``: ``source_window`` grown by ``radius`` on each side and clipped to the H x W
+    source, the pixels the unsharp-mask target of ``draw``'s crop reads."""
+    y, x, h, w = source_window(H, W, draw, oh, ow)
+    r = int(radius)
+    y0, x0 = max(0, y - r), max(0, x - r)
+    return y0, x0, min(H, y + h + r) - y0, min(W, x + w + r) - x0
+
+
+def usm_slot_bytes(inputs, batch_size: int, output_resolution, radius: int, rotate: bool) -> int:
+    """Bytes of one staging slot of UnsharpMaskDataPipeline's streamed tier: ``batch_size`` samples
+    of the largest grown window (``grown_window``) any of ``inputs`` can give under the rotations
+    ``rotate`` allows, each 256-byte aligned."""
+    oh, ow = (int(v) for v in output_resolution)
+    r = int(radius)
+    widest = 0
+    for im in inputs:
+        H, W = im.shape[:2]
+        for h, w in ((oh, ow), (ow, oh)) if rotate else ((oh, ow),):
+            widest = max(widest, _aligned(min(H, h + 2 * r) * min(W, w + 2 * r) * 3 * im.itemsize))
+    return int(batch_size) * widest
+
+
+def usm_batch(inputs, draws, output_resolution, size, blur_sigma, sharpen, windows=None, out=None):
+    """One UnsharpMaskDataPipeline batch through ``hdrnet_train_batch_usm_f32``: ``inputs[b]`` is the
+    b-th sample's source ([H, W, 3] CUDA tensor, uint8 / uint16 / float32, any mix) or, when
+    ``windows[b] = (H, W, y0, x0)`` is given, the window of an H x W source at (y0, x0) that holds
+    ``grown_window`` of its crop; ``draws[b]`` is the augmentation on the full source.  Returns
+    ``(image_input, image_output, lowres_input)`` as ``train_batch`` does, the target being the
+    unsharp mask of the input (``UnsharpMaskDataPipeline``); ``size`` None leaves out the network
+    input (returned as None) and ``out`` may then hold None in its place."""
+    sigma, amount = check_usm(blur_sigma, sharpen)
+    oh, ow = (int(v) for v in output_resolution)
+    B = len(draws)
+    if len(inputs) != B or (windows is not None and len(windows) != B):
+        raise ValueError("one input (and window) per draw")
+    descs = (_lib.UsmSample * max(B, 1))()
+    for b, (x, d) in enumerate(zip(inputs, draws)):
+        _check_source(x, f"inputs[{b}]")
+        H, W, y0, x0 = (x.shape[0], x.shape[1], 0, 0) if windows is None else (int(v) for v in windows[b])
+        descs[b] = _lib.UsmSample(x.data_ptr(), _TORCH_FMT[x.dtype], H, W, y0, x0, x.shape[0], x.shape[1],
+                                  int(bool(d.fliplr)), int(bool(d.flipud)), int(d.rot90), int(d.crop_y),
+                                  int(d.crop_x))
+    device = inputs[0].device if B else torch.device("cuda", torch.cuda.current_device())
+    shapes = ((B, oh, ow, 3), (B, oh, ow, 3), None if size is None else (B, int(size), int(size), 3))
+    if out is None:
+        out = tuple(None if sh is None else torch.empty(sh, dtype=torch.float32, device=device) for sh in shapes)
+    for t, shape in zip(out, shapes):
+        if shape is None:
+            if t is not None:
+                raise ValueError("out: no network input is written without size")
+        elif t is None or t.shape != shape or t.dtype != torch.float32 or not t.is_contiguous() or t.device != device:
+            raise ValueError(f"out: expected contiguous float32 {shape} tensors on {device}")
+    lib = _lib.load()
+    ws_bytes = lib.hdrnet_train_batch_usm_workspace_bytes(ctypes.cast(descs, ctypes.c_void_p), B, oh, ow, sigma)
+    with torch.cuda.device(device):
+        ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=device)
+        rc = lib.hdrnet_train_batch_usm_f32(
+            ctypes.cast(descs, ctypes.c_void_p), B, out[0].data_ptr(), out[1].data_ptr(),
+            0 if out[2] is None else out[2].data_ptr(), oh, ow, 0 if size is None else int(size), sigma, amount,
+            ws.data_ptr(), int(ws_bytes), torch.cuda.current_stream(device).cuda_stream)
+    _lib.check(rc, "usm_batch")
+    return out
+
+
+def unsharp_mask(image, blur_sigma, sharpen):
+    """The unsharp-mask target of a whole image: ``clip(x + sharpen * (x - G * x), 0, 1)`` with x the
+    float32 pixels of ``image`` ([H, W, 3] CUDA tensor, uint8 / uint16 / float32; integers as v / 255
+    or v / 65535), G the Gaussian of ``blur_sigma`` source pixels with reflection at the image's edges
+    (``UnsharpMaskDataPipeline``).  Returns [H, W, 3] float32: the target the pipeline gives the
+    whole-image crop with no flip or rotation, from the same kernel.  Scores ``bin/run.py`` outputs
+    against the targets a USM-trained model learned."""
+    _check_source(image, "image")
+    H, W = int(image.shape[0]), int(image.shape[1])
+    fin = torch.empty((1, H, W, 3), dtype=torch.float32, device=image.device)
+    fout = torch.empty_like(fin)
+    usm_batch([image], [Draw(0, False, False, 0, 0, 0)], (H, W), None, blur_sigma, sharpen,
+              out=(fin, fout, None))
+    return fout[0]
+
+
 def device_budget(device) -> int:
     """Free device memory on ``device`` in bytes, as the tier selection sees it."""
     return torch.cuda.mem_get_info(device)[0]
@@ -343,12 +463,17 @@ class DeviceCache:
 
 class _Staged(NamedTuple):
     """A batch in device slot ``slot``: each sample's (input, target) window views and its draw with
-    the crop at the window's origin; ``uploaded`` is the event of the slot's copy."""
+    the crop at the window's origin; ``uploaded`` is the event of the slot's copy.  Without targets
+    (UnsharpMaskDataPipeline) each view is the crop's window grown by the blur radius, ``draws`` keep
+    the crop on the full source and ``windows`` holds each view's ``(H, W, y0, x0)``.  ``nbytes``: the
+    bytes the slot's copy moved."""
     slot: int
     inputs: list
     targets: list
     draws: list
     uploaded: object
+    windows: list = None
+    nbytes: int = 0
 
 
 class HostStream:
@@ -359,12 +484,17 @@ class HostStream:
     ``consumed`` event recorded on the consumer's stream; the copy stream waits on it), and a pinned
     slot only after its previous upload has completed (the producer waits on the host)."""
 
-    def __init__(self, inputs, targets, sampler, output_resolution, device, nthreads=1):
+    def __init__(self, inputs, targets, sampler, output_resolution, device, nthreads=1, radius=None):
         self.inputs, self.targets, self.sampler = inputs, targets, sampler
         self.oh, self.ow = (int(v) for v in output_resolution)
         self.device = device
-        self.slot_bytes = slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)}, sampler.shard_size,
-                                     output_resolution)
+        self.radius = radius        # targets None: stage each crop's window grown by this
+        if targets is None:
+            self.slot_bytes = usm_slot_bytes(inputs, sampler.shard_size, output_resolution, radius,
+                                             sampler.rotate)
+        else:
+            self.slot_bytes = slot_bytes({(a.dtype, b.dtype) for a, b in zip(inputs, targets)},
+                                         sampler.shard_size, output_resolution)
         with torch.cuda.device(device):
             self.copy_stream = torch.cuda.Stream(device)
             with torch.cuda.stream(self.copy_stream):     # the blocks belong to the stream that writes them
@@ -392,6 +522,8 @@ class HostStream:
         """Copy batch ``step``'s windows (the sampler's shard of them) into pinned slot ``slot`` and
         upload it to device slot ``slot`` on the copy stream."""
         draws = self.sampler.shard_draws(step)
+        if self.targets is None:
+            return self._pack_grown(slot, draws)
         layout, off = [], 0
         for d in draws:
             a, b = self.inputs[d.index], self.targets[d.index]
@@ -424,7 +556,42 @@ class HostStream:
             inputs.append(dev[oa:oa + h * w * 3 * a.itemsize].view(getattr(torch, a.dtype.name)).view(h, w, 3))
             targets.append(dev[ob:ob + h * w * 3 * b.itemsize].view(getattr(torch, b.dtype.name)).view(h, w, 3))
             crops.append(d._replace(crop_y=0, crop_x=0))
-        return _Staged(slot, inputs, targets, crops, self.uploaded[slot])
+        return _Staged(slot, inputs, targets, crops, self.uploaded[slot], None, off)
+
+    def _pack_grown(self, slot: int, draws) -> _Staged:
+        """``_pack`` without targets: each sample's crop window grown by ``radius`` on each side and
+        clipped to the source (``grown_window``), the draw unchanged."""
+        layout, off = [], 0
+        for d in draws:
+            a = self.inputs[d.index]
+            win = grown_window(a.shape[0], a.shape[1], d, self.oh, self.ow, self.radius)
+            layout.append((d, win, off))
+            off += _aligned(win[2] * win[3] * 3 * a.itemsize)
+        self.uploaded[slot].synchronize()                  # the pinned slot's last upload has completed
+        host = self.pinned[slot].numpy()
+
+        def copy(item):
+            d, (y0, x0, h, w), o = item
+            src = self.inputs[d.index]
+            np.copyto(host[o:o + h * w * 3 * src.itemsize].view(src.dtype).reshape(h, w, 3),
+                      src[y0:y0 + h, x0:x0 + w])
+
+        t0 = time.perf_counter()
+        list(self.pool.map(copy, layout))
+        self.pack_seconds += time.perf_counter() - t0
+        self.packed += 1
+        with torch.cuda.device(self.device), torch.cuda.stream(self.copy_stream):
+            if self.consumed[slot] is not None:
+                self.copy_stream.wait_event(self.consumed[slot])
+            self.dev[slot][:off].copy_(self.pinned[slot][:off], non_blocking=True)
+            self.uploaded[slot].record(self.copy_stream)
+        dev = self.dev[slot]
+        inputs, windows = [], []
+        for d, (y0, x0, h, w), o in layout:
+            a = self.inputs[d.index]
+            inputs.append(dev[o:o + h * w * 3 * a.itemsize].view(getattr(torch, a.dtype.name)).view(h, w, 3))
+            windows.append((a.shape[0], a.shape[1], y0, x0))
+        return _Staged(slot, inputs, None, list(draws), self.uploaded[slot], windows, off)
 
     def _produce(self):
         while True:
@@ -582,3 +749,82 @@ class ImageFilesDataPipeline:
 
     def __exit__(self, *exc):
         self.close()
+
+
+class UnsharpMaskDataPipeline(ImageFilesDataPipeline):
+    """Training data from input images alone: the target is an unsharp mask of the input.
+
+    The reference's ``scripts/usm/*.sh`` recipes name this pipeline (``--data_pipeline
+    UnsharpMaskDataPipeline --blur_sigma S --sharpen A``), but its ``data_pipeline.py`` does not define
+    it and its ``train.py`` has neither flag; what follows is this project's definition.  With x the
+    float32 input exactly as ``image_input`` holds it (v / 255, v / 65535, or float32 as stored):
+
+    * b = G * x per channel, G the separable Gaussian of standard deviation ``blur_sigma`` source
+      pixels: radius r = int(4 sigma + 0.5), weights exp(-k^2 / 2 sigma^2) for |k| <= r normalised to
+      sum 1, along source x, then source y, with half-sample symmetric reflection (d c b a | a b c d,
+      repeated when r reaches the extent) at the source image's edges: scipy's
+      ``ndimage.gaussian_filter1d(..., mode="reflect", truncate=4.0)`` on each axis.
+    * target = clip(x + sharpen * (x - b), 0, 1), in the range an image-file target has.
+    * The target is a function of the un-augmented source pixel: the crop selects pixels (its edges
+      get no boundary effects) and the flips and rot90 move them, so this equals augmenting first.
+    * ``image_input`` and ``lowres_input`` are ``ImageFilesDataPipeline``'s for the same input and draw.
+
+    0 < ``blur_sigma`` <= 32 and a finite ``sharpen``, else ValueError before any file is read.
+    Takes ``ImageFilesDataPipeline``'s keywords; reads ``filelist.txt`` and ``input/`` only.  The
+    device tier caches the inputs alone (``dataset_bytes`` counts them); the streamed tier stages
+    each sample's crop window grown by r on each side and clipped to the source, and gives the
+    device tier's batches bit for bit.  One kernel, ``hdrnet_train_batch_usm_f32``
+    (csrc/usm_batch.cu), builds each batch."""
+
+    def __init__(self, path, batch_size=32, output_resolution=(1080, 1920), shuffle=False, fliplr=False,
+                 flipud=False, rotate=False, random_crop=False, params=None, nthreads=1, seed=0, device=None,
+                 memory_margin=MEMORY_MARGIN, shard=(0, 1), blur_sigma=None, sharpen=None):
+        self.blur_sigma, self.sharpen = check_usm(blur_sigma, sharpen)
+        self.radius = usm_radius(self.blur_sigma)
+        check_shard(shard, batch_size)
+        self.path = path
+        self.batch_size = int(batch_size)
+        self.output_resolution = [int(v) for v in output_resolution]
+        self.net_input_size = int((params or {}).get("net_input_size", 256))
+        names, inputs, dirname = load_inputs(path, nthreads)
+        check_inputs(names, inputs, dirname, self.output_resolution, rotate)
+        self.names = names
+        self.nsamples = len(names)
+        self.sampler = Sampler([a.shape[:2] for a in inputs], batch_size, self.output_resolution, shuffle,
+                               fliplr, flipud, rotate, random_crop, seed, shard)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.dataset_bytes = cache_bytes(inputs)
+        self.staging_bytes = STREAM_SLOTS * usm_slot_bytes(inputs, self.sampler.shard_size, self.output_resolution,
+                                                           self.radius, rotate)
+        self.tier = choose_tier(self.dataset_bytes, self.staging_bytes, self.device, memory_margin)
+        self.stream = None
+        self.targets = None
+        if self.tier == "device":
+            self.cache = DeviceCache(inputs, self.device)
+            self.inputs = self.cache.images
+            log.info("%s: %d inputs, %.1f MB on %s (unsharp-mask targets: sigma %g, sharpen %g)", dirname,
+                     self.nsamples, self.cache.nbytes / 1e6, self.device, self.blur_sigma, self.sharpen)
+        else:
+            self.stream = HostStream(inputs, None, self.sampler, self.output_resolution, self.device, nthreads,
+                                     radius=self.radius)
+            log.info("%s: %d inputs, %.1f MB: more than the %.1f MB of %s's free memory less the %.1f MB kept "
+                     "for training, so they stay on the host and each batch's crops, grown by the blur radius %d, "
+                     "are streamed through %d staging slots of %.1f MB", dirname, self.nsamples,
+                     self.dataset_bytes / 1e6, device_budget(self.device) / 1e6, self.device, memory_margin / 1e6,
+                     self.radius, STREAM_SLOTS, self.stream.slot_bytes / 1e6)
+
+    def batch(self, step: int) -> dict:
+        if self.stream is None:
+            draws = self.sampler.shard_draws(step)
+            fin, fout, low = usm_batch([self.inputs[d.index] for d in draws], draws, self.output_resolution,
+                                       self.net_input_size, self.blur_sigma, self.sharpen)
+            return {"image_input": fin, "image_output": fout, "lowres_input": low}
+        item = self.stream.take(step)
+        stream = torch.cuda.current_stream(self.device)
+        stream.wait_event(item.uploaded)
+        try:
+            fin, fout, low = usm_batch(item.inputs, item.draws, self.output_resolution, self.net_input_size,
+                                       self.blur_sigma, self.sharpen, windows=item.windows)
+        finally:
+            self.stream.consumed_by(item, stream)
+        return {"image_input": fin, "image_output": fout, "lowres_input": low}

@@ -587,6 +587,50 @@ HDRNET_API int hdrnet_train_batch_f32(const hdrnet_train_sample* samples, int B,
                                       void* stream);
 
 /*
+ * One training batch of UnsharpMaskDataPipeline: the target is computed from the input.  The
+ * reference's usm/ scripts name this pipeline but its sources do not define it; this is the
+ * project's definition.  With x the float32 input pixel (converted as hdrnet_train_batch_f32 does)
+ *   b = G_sigma * x   per channel: the separable Gaussian of scipy.ndimage.gaussian_filter1d
+ *                     (truncate 4.0: radius r = int(4 sigma + 0.5), weights exp(-k^2 / 2 sigma^2)
+ *                     normalised to sum 1) along source x, then source y, with half-sample
+ *                     symmetric reflection (d c b a | a b c d, repeated) at the SOURCE's edges
+ *   fullres_out = clip(x + sharpen (x - b), 0, 1)
+ * computed in source coordinates: a source pixel's target does not depend on the draw, and the
+ * flips, rot90 and crop (hdrnet_train_batch_f32's) only move pixels.  fullres_in and lowres_in are
+ * hdrnet_train_batch_f32's, bit for bit; either may be NULL (not written; S is then ignored).
+ *
+ * A sample's buffer holds a window of its source: rows [y0, y0 + h), columns [x0, x0 + w) of the
+ * full H x W source, row pitch w pixels.  It must cover the crop's source rectangle grown by r on
+ * each side and clipped to [0, H) x [0, W) (the whole source always does).  The flips, rot90 and
+ * crop origin are given on the full source's rotated extent.  Sums run in float64 in a fixed tap
+ * order, no atomics: bitwise the same from run to run.  0 < sigma <= 32 (so r <= 128); sharpen
+ * finite.  The workspace (4-byte aligned) holds float32 rows of the horizontal pass; its size is
+ * hdrnet_train_batch_usm_workspace_bytes (0 for B = 0 or arguments the call refuses).  `samples`
+ * is a HOST array read before the call returns.  Errors, all before any launch:
+ * HDRNET_E_NULL_POINTER for a NULL descriptor array, input, fullres_out or workspace;
+ * HDRNET_E_BAD_SHAPE for B < 0, oh / ow < 1, S < 1 with lowres_in, a bad sigma or sharpen, H or
+ * W <= 0, k outside 0..3, a crop outside the rotated source, a window outside the source or not
+ * covering the grown crop rectangle, or a short or misaligned workspace; HDRNET_E_UNSUPPORTED for
+ * an unknown format; HDRNET_E_TOO_LARGE for grids past the launch limits.  B = 0 succeeds.
+ */
+typedef struct hdrnet_usm_sample {
+  const void* input;    /* the window [h, w, 3] in input_fmt (HDRNET_PX_*), device memory */
+  int input_fmt;
+  int H, W;             /* the full source's extent                                      */
+  int y0, x0, h, w;     /* the window the buffer holds, in source pixels                 */
+  int fliplr, flipud;   /* nonzero: flip                                                 */
+  int rot90;            /* k in 0..3                                                     */
+  int crop_y, crop_x;   /* crop origin on the full source's rotated extent               */
+} hdrnet_usm_sample;
+
+HDRNET_API size_t hdrnet_train_batch_usm_workspace_bytes(const hdrnet_usm_sample* samples, int B, int oh,
+                                                          int ow, double sigma);
+HDRNET_API int hdrnet_train_batch_usm_f32(const hdrnet_usm_sample* samples, int B, float* fullres_in,
+                                          float* fullres_out, float* lowres_in, int oh, int ow, int S,
+                                          double sigma, double sharpen, void* workspace,
+                                          size_t workspace_bytes, void* stream);
+
+/*
  * Host-buffer path (what a CPU-tensor caller of the reference op gets: TF copies feeds to
  * the GPU and fetches back, hdrnet/bin/run.py:185).  A context owns device staging buffers
  * and streams; the call splits the batch into row bands, and pipelines H2D copy -> kernel

@@ -839,8 +839,10 @@ template <class GuideFn, int kTexChunks = 0>
 static int launch_tma(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream, int in_fmt = kPxF32,
                       int out_fmt = kPxF32) {
   if constexpr (GuideFn::kFromInput) {
-    // plan.threads == 512: 64 registers per thread (no spills), 32 warps per SM
-    if (a.p.threads == 512) return launch_tma_occ<GuideFn, kTexChunks, 2, 512>(a, fn, stream);
+    // the texture-assisted form of the op API: 512 threads, 64 registers per thread (no spills), 32
+    // warps per SM (plan_slice_apply gives it no other plan)
+    if constexpr (kTexChunks > 0) return launch_tma_occ<GuideFn, kTexChunks, 2, kTexThreads>(a, fn, stream);
+    else return launch_tma_occ<GuideFn, 0, 2>(a, fn, stream);
   } else {
     // The fused-guide forms are issue-bound and need their registers: 256 threads x 2 CTAs.
     // (chosen against 256 x 3 and 512 x 2 on the previous target; not re-tuned on H100).  Integer
@@ -853,9 +855,9 @@ static int launch_tma(const TmaArgs& a, const GuideFn& fn, cudaStream_t stream, 
       return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU8, kPxU16>(a, fn, stream);
     if (in_fmt == kPxU16 && out_fmt == kPxU16)
       return launch_tma_occ<GuideFn, kTexChunks, 2, kTmaThreads, kPxU16, kPxU16>(a, fn, stream);
+    if (in_fmt != kPxF32 || out_fmt != kPxF32) return HDRNET_E_UNSUPPORTED;
+    return launch_tma_occ<GuideFn, kTexChunks, 2>(a, fn, stream);
   }
-  if (in_fmt != kPxF32 || out_fmt != kPxF32) return HDRNET_E_UNSUPPORTED;
-  return launch_tma_occ<GuideFn, kTexChunks, 2>(a, fn, stream);
 }
 
 // Texture objects over caller workspaces.  Creating one is a host-side driver call that should
@@ -1130,10 +1132,12 @@ static int plan_slice_apply(const SliceGeom& g, int n_in, int n_out, int has_off
     f->fused_async = mode == 1 &&
                      make_tma_plan(g, max_smem, sms, &fplan, true, kFusedAsyncMathThreads, in_fmt, out_fmt) &&
                      fplan.resident == kFusedAsyncResident && fplan.stages >= 3;
+    // the block-synchronous texture form: 512 threads for the op API, 256 for fused guides.  It holds
+    // no slab region, so it fits wherever the row plan does (at twice the row plan's threads too)
     if (f->fused_async) {
       f->p = fplan;
     } else if (!make_tma_plan(g, max_smem, sms, &f->p, true, mode != 0 ? kTmaThreads : kTexThreads, in_fmt, out_fmt)) {
-      f->p = plan;   // the block-synchronous texture form: 512 threads for the op API, 256 for fused guides
+      return HDRNET_E_UNSUPPORTED;
     }
   }
   // launch threads: the issuer-warp forms add the issuer warp, and the slab warp where there is one

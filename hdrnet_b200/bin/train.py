@@ -118,7 +118,15 @@ Deliberate differences from the reference:
   step size.  With eps = 1e-8 the two differ only while sqrt(v) is of the order of eps.
 * No queue runners, summaries or TF event files: batches are built on the device when needed and
   the scalars go to ``train_log.jsonl``.  The random streams are not TF's (data_pipeline.py).
-* The decoded dataset must fit in host memory: every pair is decoded once at start-up.
+* Every file is decoded once at start-up.  By default the decoded dataset is held in host memory, so
+  it must fit there, and every rank holds its own copy.  ``--decoded_cache DIR`` instead decodes each
+  file once into an on-disk cache at DIR (``data_pipeline.DecodedCache``) and maps its entries: the
+  page cache holds one copy for all ranks, a dataset larger than RAM is paged in from disk as the
+  crops read it, and a later run or resume opens the entries without decoding.  Under ``torchrun``
+  the ranks split the decoding of missing entries, for the training and the eval set.  It applies
+  to ``data_dir`` and ``--eval_data_dir`` with either pipeline, gives the same batches and so the
+  same checkpoints, and is not a model parameter: it is not written to ``params.json`` or to the
+  checkpoints, and a resume may add or drop it.
 """
 from __future__ import annotations
 
@@ -197,6 +205,9 @@ def build_parser() -> argparse.ArgumentParser:
                                "pixels (0 < S <= 32).")
     data_grp.add_argument("--sharpen", default=None, type=float,
                           help="UnsharpMaskDataPipeline: the target is clip(x + sharpen * (x - blur(x)), 0, 1).")
+    data_grp.add_argument("--decoded_cache", default=None, type=str, metavar="DIR",
+                          help="decode each image once into this on-disk cache and map it, instead of holding the "
+                               "decoded dataset in memory (data_dir and --eval_data_dir; shared by ranks and runs).")
 
     model_grp = parser.add_argument_group("model_params")
     model_grp.add_argument("--model_name", default=models.__all__[0], type=str, help="classname of the model to use.",
@@ -401,21 +412,29 @@ class Trainer:
                      "restored" if self.step else "initial")
         self.usm = usm_values(args)
         if self.usm is None:
-            pipeline, usm_kw = data_pipeline.ImageFilesDataPipeline, {}
+            pipeline, data_kw = data_pipeline.ImageFilesDataPipeline, {}
         else:
             pipeline = data_pipeline.UnsharpMaskDataPipeline
-            usm_kw = {"blur_sigma": self.usm[0], "sharpen": self.usm[1]}
+            data_kw = {"blur_sigma": self.usm[0], "sharpen": self.usm[1]}
             log.info("targets: unsharp masks of the inputs (blur_sigma %g, sharpen %g)", *self.usm)
+        if getattr(args, "decoded_cache", None) is not None:
+            data_kw["decoded_cache"] = args.decoded_cache
         self.train_data = pipeline(
             args.data_dir, batch_size=args.batch_size, output_resolution=args.output_resolution, shuffle=True,
             fliplr=args.fliplr, flipud=args.flipud, rotate=args.rotate, random_crop=args.random_crop,
             params=params, nthreads=args.data_threads, seed=args.seed, device=self.device,
-            shard=(self.rank, self.world), **usm_kw)
+            shard=(self.rank, self.world), **data_kw)
         self.eval_data = None
         if args.eval_data_dir is not None:
             self.eval_data = pipeline(
                 args.eval_data_dir, batch_size=1, output_resolution=args.output_resolution, shuffle=False,
-                params=params, nthreads=1, device=self.device, **usm_kw)
+                params=params, nthreads=args.data_threads if "decoded_cache" in data_kw else 1, device=self.device,
+                **data_kw)
+        for data in (self.train_data, self.eval_data):
+            dc = getattr(data, "decoded_cache", None)
+            if dc is not None:
+                log.info("%s: decoded cache %s: %d entries valid, %d built, %.1f MB mapped", data.path,
+                         dc.directory, dc.valid, dc.built, dc.nbytes / 1e6)
         self.p = dict(params, weights=self.weights)
         if args.train_guide:
             self.p["guide_grad"] = True

@@ -39,23 +39,33 @@ Deliberate differences:
   (data_pipeline.py:166).  They are equal at the default.
 * Each file keeps its own pixel format; the reference decides from the first file of each folder.
 * No queue runners: a batch is ready when its kernel has run.
-* The whole dataset must fit in host memory: it is decoded once at start-up, not on demand.
+* Every file is decoded once, not per sample.  By default the decoded pixels are held in process
+  memory, so the dataset must fit in host memory.  With ``decoded_cache=DIR`` each file is decoded
+  once into an entry of an on-disk cache (``DecodedCache``) and the pipeline holds ``np.memmap``
+  views of the entries: the page cache keeps one copy for every process of the host, the kernel
+  pages windows in from disk when the dataset is larger than RAM, and a later run opens the entries
+  without decoding.
 """
 from __future__ import annotations
 
 import concurrent.futures
 import ctypes
 import functools
+import hashlib
 import logging
 import os
+import resource
+import struct
 import threading
 import time
 from typing import NamedTuple
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
-from . import _lib
+from . import _lib, parallel
+from .checkpoint import crc32c
 
 __all__ = ["ImageFilesDataPipeline", "UnsharpMaskDataPipeline"]
 
@@ -103,23 +113,205 @@ def decode_image(path: str) -> np.ndarray:
     return np.ascontiguousarray(im)
 
 
-def load_pairs(path: str, nthreads: int = 1):
-    """(names, inputs, targets, data directory): every pair named by the file list, decoded."""
+class DecodedCache:
+    """A directory of decoded images: one entry file per source image, opened as ``np.memmap``.
+
+    An entry is named by the first 32 hex digits of the SHA-256 of the source's absolute path, plus
+    ``.px``, so one directory serves any number of datasets.  It holds a ``HEADER_BYTES`` header,
+    then exactly what ``decode_image`` returns: [H, W, 3] in C order, little-endian, so the pixels
+    start page-aligned for every format.  The header holds, in order (little-endian):
+
+    * the magic ``b"HDRNPXC\\0"`` and the u32 format ``VERSION``;
+    * the u32 pixel format (``_lib.PX_U8 / PX_U16 / PX_F32``), u32 H and u32 W;
+    * the source file's u64 size and i64 ``st_mtime_ns``;
+    * the u32 length of the source's absolute path, then the path;
+    * a u32 CRC-32C (``checkpoint.crc32c``) of everything before it; zeros to ``HEADER_BYTES``.
+
+    An entry is valid only when the magic, version and CRC match, the padding is zero, the recorded
+    path is the source's, the source's size and mtime are the recorded ones, and the file is exactly
+    header plus pixel bytes.  Anything else (a truncated file, a damaged header, another version, a
+    changed or touched source, a digest shared with another path) is treated as missing and rebuilt.
+    The pixels carry no checksum: their integrity is left to the filesystem, as for the source
+    files, since checking them would cost a full read of the dataset at every start.
+
+    An entry is written to a name unique to the writing process and thread, made durable, then
+    renamed into place (``os.replace``), so processes building one cache at once are safe and no
+    reader sees a partial entry; leftover temporary files (``.*.tmp``) are never read as entries.  A
+    read-only directory works while its entries are valid; a missing or invalid one there raises the
+    OS error, naming the directory.
+
+    ``open`` maps every entry copy-on-write (``mode="c"``): the arrays are writable as numpy and
+    torch expect, yet nothing is ever written to the files, and pages read stay shared page-cache
+    pages rather than process memory.  ``valid``, ``built`` and ``nbytes`` count what ``open`` found
+    valid, what it decoded and wrote, and the pixel bytes it mapped."""
+
+    HEADER_BYTES = 4096
+    VERSION = 1
+    MAGIC = b"HDRNPXC\0"
+    _HEAD = struct.Struct("<8sIIIIQqI")      # magic, version, format, H, W, source size, mtime_ns, path length
+    _DTYPES = {_lib.PX_U8: np.dtype("<u1"), _lib.PX_U16: np.dtype("<u2"), _lib.PX_F32: np.dtype("<f4")}
+
+    def __init__(self, directory):
+        self.directory = os.path.abspath(os.fspath(directory))
+        self.valid = self.built = self.nbytes = 0
+
+    def entry_path(self, source: str) -> str:
+        """The entry file of ``source`` (any path; its absolute path names the entry)."""
+        digest = hashlib.sha256(os.fsencode(os.path.abspath(source))).hexdigest()[:32]
+        return os.path.join(self.directory, digest + ".px")
+
+    @classmethod
+    def header(cls, fmt: int, H: int, W: int, size: int, mtime_ns: int, source: str) -> bytes:
+        path = os.fsencode(source)
+        body = cls._HEAD.pack(cls.MAGIC, cls.VERSION, fmt, H, W, size, mtime_ns, len(path)) + path
+        if len(body) + 4 > cls.HEADER_BYTES:
+            raise ValueError(f"{source}: the path is too long for a decoded-cache entry header")
+        return (body + struct.pack("<I", crc32c(body))).ljust(cls.HEADER_BYTES, b"\0")
+
+    def entry(self, source: str):
+        """``(dtype, H, W)`` of ``source``'s entry when it is valid, else None."""
+        source = os.path.abspath(source)
+        try:
+            st = os.stat(source)
+            with open(self.entry_path(source), "rb") as f:
+                head = f.read(self.HEADER_BYTES)
+                length = os.fstat(f.fileno()).st_size
+        except OSError:
+            return None
+        if len(head) != self.HEADER_BYTES:
+            return None
+        magic, version, fmt, H, W, size, mtime_ns, n = self._HEAD.unpack_from(head)
+        end = self._HEAD.size + n
+        if magic != self.MAGIC or version != self.VERSION or end + 4 > self.HEADER_BYTES:
+            return None
+        if crc32c(head[:end]) != struct.unpack_from("<I", head, end)[0] or head[end + 4:].strip(b"\0"):
+            return None
+        dtype = self._DTYPES.get(fmt)
+        if (dtype is None or head[self._HEAD.size:end] != os.fsencode(source) or size != st.st_size
+                or mtime_ns != st.st_mtime_ns or length != self.HEADER_BYTES + H * W * 3 * dtype.itemsize):
+            return None
+        return dtype, H, W
+
+    def build(self, source: str) -> None:
+        """Decode ``source`` and write its entry (temporary name, then ``os.replace``)."""
+        source = os.path.abspath(source)
+        st = os.stat(source)                 # before decoding: a source changed meanwhile is rebuilt next time
+        im = decode_image(source)
+        head = self.header(_FMT[im.dtype], im.shape[0], im.shape[1], st.st_size, st.st_mtime_ns, source)
+        entry = self.entry_path(source)
+        tmp = os.path.join(self.directory,
+                           f".{os.path.basename(entry)}.{os.getpid()}.{threading.get_ident()}.tmp")
+        try:
+            f = open(tmp, "wb")
+        except OSError as e:
+            raise type(e)(e.errno, f"decoded cache {self.directory}: cannot write the entry of {source}: "
+                                   f"{e.strerror}") from e
+        try:
+            with f:
+                f.write(head)
+                f.write(np.ascontiguousarray(im, im.dtype.newbyteorder("<")).data)
+                f.flush()
+                os.fsync(f.fileno())
+            os.replace(tmp, entry)
+        except BaseException:
+            try:
+                os.unlink(tmp)
+            except OSError:
+                pass
+            raise
+
+    def open(self, sources, nthreads: int = 1) -> list:
+        """One ``np.memmap`` per source, each equal to ``decode_image(source)`` bit for bit; missing
+        or invalid entries are built first on ``nthreads`` threads.
+
+        Under a ``torch.distributed`` process group every rank calls this with the same sources: the
+        ranks first agree that each has checked the entries, then the k-th missing entry (in the
+        order of ``sources``) is built by rank k mod world, and the ranks meet again, carrying any
+        rank's failure, before each opens every entry.  So a dataset is decoded once over the ranks
+        whatever the pipeline's ``shard``."""
+        os.makedirs(self.directory, exist_ok=True)
+        unique = list(dict.fromkeys(os.path.abspath(s) for s in sources))
+        found = {s: self.entry(s) for s in unique}
+        missing = [s for s in unique if found[s] is None]
+        rank, world = (dist.get_rank(), dist.get_world_size()) if parallel.world_size() > 1 else (0, 1)
+        if world > 1:
+            parallel.sum_over_ranks([0.0])       # every rank has checked before any builds: one split
+        error = None
+        try:
+            self._build_all(missing[rank::world], nthreads)
+        except BaseException as e:
+            error = e
+        if world > 1:
+            failed = parallel.sum_over_ranks([float(error is not None)])[0]
+            if error is None and failed:
+                raise RuntimeError(f"decoded cache {self.directory}: another rank failed to build its entries")
+        if error is not None:
+            raise error
+        for s in missing:
+            found[s] = self.entry(s)
+        rebuild = [s for s in missing if found[s] is None]      # another rank's share, built again here
+        self._build_all(rebuild, nthreads)
+        for s in rebuild:
+            found[s] = self.entry(s)
+            if found[s] is None:
+                raise RuntimeError(f"decoded cache {self.directory}: the entry of {s} is not valid after it was "
+                                   "written (was it changed meanwhile?)")
+        _fd_headroom(len(unique))                # each map holds a file descriptor
+        maps = {}
+        for s in unique:
+            dtype, H, W = found[s]
+            maps[s] = np.memmap(self.entry_path(s), dtype=dtype, mode="c", offset=self.HEADER_BYTES,
+                                shape=(H, W, 3))
+        self.valid += len(unique) - len(missing)
+        self.nbytes += sum(m.nbytes for m in maps.values())
+        return [maps[os.path.abspath(s)] for s in sources]
+
+    def _build_all(self, sources, nthreads):
+        if sources:
+            with concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads))) as ex:
+                list(ex.map(self.build, sources))
+            self.built += len(sources)
+
+
+def _fd_headroom(n: int) -> None:
+    """Raise this process's soft limit on open files, up to its hard limit, so that ``n`` more
+    descriptors fit (each ``np.memmap`` keeps one open); OSError when the hard limit is too low."""
+    soft, hard = resource.getrlimit(resource.RLIMIT_NOFILE)
+    need = len(os.listdir("/proc/self/fd")) + int(n) + 64
+    if soft != resource.RLIM_INFINITY and soft < need:
+        if hard != resource.RLIM_INFINITY and hard < need:
+            raise OSError(f"mapping {n} decoded-cache entries needs {need} open files; the limit is {hard}")
+        resource.setrlimit(resource.RLIMIT_NOFILE, (need, hard))
+
+
+def _decoded(files, nthreads, cache):
+    """Each of ``files`` decoded, or, with ``cache`` (a directory or a ``DecodedCache``), mapped
+    from the cache's entries."""
+    if cache is None:
+        with concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads))) as ex:
+            return list(ex.map(decode_image, files))
+    if not isinstance(cache, DecodedCache):
+        cache = DecodedCache(cache)
+    return cache.open(files, nthreads)
+
+
+def load_pairs(path: str, nthreads: int = 1, cache=None):
+    """(names, inputs, targets, data directory): every pair named by the file list, decoded; with
+    ``cache`` (a directory or a ``DecodedCache``) as ``np.memmap`` views of its entries instead."""
     dirname, filelist = data_paths(path)
     names = read_filelist(filelist)
     files = [os.path.join(dirname, sub, n) for n in names for sub in ("input", "output")]
-    with concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads))) as ex:
-        ims = list(ex.map(decode_image, files))
+    ims = _decoded(files, nthreads, cache)
     return names, ims[0::2], ims[1::2], dirname
 
 
-def load_inputs(path: str, nthreads: int = 1):
-    """(names, inputs, data directory): every input named by the file list, decoded; ``output/`` is
-    not read (UnsharpMaskDataPipeline computes its targets)."""
+def load_inputs(path: str, nthreads: int = 1, cache=None):
+    """(names, inputs, data directory): every input named by the file list, decoded (or mapped from
+    ``cache``, as ``load_pairs``); ``output/`` is not read (UnsharpMaskDataPipeline computes its
+    targets)."""
     dirname, filelist = data_paths(path)
     names = read_filelist(filelist)
-    with concurrent.futures.ThreadPoolExecutor(max(1, int(nthreads))) as ex:
-        ims = list(ex.map(decode_image, [os.path.join(dirname, "input", n) for n in names]))
+    ims = _decoded([os.path.join(dirname, "input", n) for n in names], nthreads, cache)
     return names, ims, dirname
 
 
@@ -686,17 +878,26 @@ class ImageFilesDataPipeline:
     ``shard=(rank, world)``: one rank of a data-parallel run.  ``batch_size`` is the whole batch, and
     ``batch(step)`` holds only this rank's B / world rows of it (``Sampler.shard_draws``), on either
     tier; the streamed tier packs and uploads only their windows.  ValueError, before any file is
-    read, when ``world`` does not divide ``batch_size``."""
+    read, when ``world`` does not divide ``batch_size``.
+
+    ``decoded_cache=DIR``: the files are decoded once into the ``DecodedCache`` at DIR (shared with
+    other datasets, runs and ranks) and the pipeline holds ``np.memmap`` views of its entries instead
+    of decoded arrays, on either tier, with the same batches.  ``self.decoded_cache`` then counts the
+    entries found valid, those built, and the bytes mapped; without it, it is None."""
 
     def __init__(self, path, batch_size=32, output_resolution=(1080, 1920), shuffle=False, fliplr=False,
                  flipud=False, rotate=False, random_crop=False, params=None, nthreads=1, seed=0, device=None,
-                 memory_margin=MEMORY_MARGIN, shard=(0, 1)):
+                 memory_margin=MEMORY_MARGIN, shard=(0, 1), decoded_cache=None):
         check_shard(shard, batch_size)
         self.path = path
         self.batch_size = int(batch_size)
         self.output_resolution = [int(v) for v in output_resolution]
         self.net_input_size = int((params or {}).get("net_input_size", 256))
-        names, inputs, targets, dirname = load_pairs(path, nthreads)
+        self.decoded_cache = None if decoded_cache is None else DecodedCache(decoded_cache)
+        if self.decoded_cache is None:
+            names, inputs, targets, dirname = load_pairs(path, nthreads)
+        else:
+            names, inputs, targets, dirname = load_pairs(path, nthreads, cache=self.decoded_cache)
         check_pairs(names, inputs, targets, dirname, self.output_resolution, rotate)
         self.names = names
         self.nsamples = len(names)
@@ -770,7 +971,8 @@ class UnsharpMaskDataPipeline(ImageFilesDataPipeline):
     * ``image_input`` and ``lowres_input`` are ``ImageFilesDataPipeline``'s for the same input and draw.
 
     0 < ``blur_sigma`` <= 32 and a finite ``sharpen``, else ValueError before any file is read.
-    Takes ``ImageFilesDataPipeline``'s keywords; reads ``filelist.txt`` and ``input/`` only.  The
+    Takes ``ImageFilesDataPipeline``'s keywords (``decoded_cache`` included); reads ``filelist.txt``
+    and ``input/`` only.  The
     device tier caches the inputs alone (``dataset_bytes`` counts them); the streamed tier stages
     each sample's crop window grown by r on each side and clipped to the source, and gives the
     device tier's batches bit for bit.  One kernel, ``hdrnet_train_batch_usm_f32``
@@ -778,7 +980,7 @@ class UnsharpMaskDataPipeline(ImageFilesDataPipeline):
 
     def __init__(self, path, batch_size=32, output_resolution=(1080, 1920), shuffle=False, fliplr=False,
                  flipud=False, rotate=False, random_crop=False, params=None, nthreads=1, seed=0, device=None,
-                 memory_margin=MEMORY_MARGIN, shard=(0, 1), blur_sigma=None, sharpen=None):
+                 memory_margin=MEMORY_MARGIN, shard=(0, 1), blur_sigma=None, sharpen=None, decoded_cache=None):
         self.blur_sigma, self.sharpen = check_usm(blur_sigma, sharpen)
         self.radius = usm_radius(self.blur_sigma)
         check_shard(shard, batch_size)
@@ -786,7 +988,11 @@ class UnsharpMaskDataPipeline(ImageFilesDataPipeline):
         self.batch_size = int(batch_size)
         self.output_resolution = [int(v) for v in output_resolution]
         self.net_input_size = int((params or {}).get("net_input_size", 256))
-        names, inputs, dirname = load_inputs(path, nthreads)
+        self.decoded_cache = None if decoded_cache is None else DecodedCache(decoded_cache)
+        if self.decoded_cache is None:
+            names, inputs, dirname = load_inputs(path, nthreads)
+        else:
+            names, inputs, dirname = load_inputs(path, nthreads, cache=self.decoded_cache)
         check_inputs(names, inputs, dirname, self.output_resolution, rotate)
         self.names = names
         self.nsamples = len(names)

@@ -58,6 +58,13 @@ levels' moving averages get no Adam slots, go into every checkpoint and are rest
 evaluation and ``bin/run.py`` run the guide-fused inference form on them.  The pyramid without both
 flags would train through its inference form, which is not differentiated, so it is refused.
 
+``HDRNetGaussianPyr`` is that pyramid with ``HDRNetCurves``' guide at every level
+(``inference/guide/level_{0,1,2}/{ccm, ccm_bias, shifts, slopes, channel_mixing/*}``), the model the
+reference's ``*_gpyr*.sh`` recipes name (models.HDRNetGaussianPyr defines it).  It trains as
+``HDRNetCurves`` does: ``--nobatch_norm``, with ``--train_guide`` its three curves guides too, without it
+the three held fixed.  Its guides have no batch norm, so ``--guide_batch_stats`` is refused with
+``ValueError`` and ``--batch_norm --coefficient_batch_stats`` does not need it.
+
 ``--batch_norm --coefficient_batch_stats`` trains the coefficient network's batch norm as the
 reference's ``--batch_norm`` does (train.py:92-115): each step runs ``inference(..., is_training=True)``
 with the batch-norm layers normalised by the batch's statistics (the whole batch's under a process
@@ -211,7 +218,7 @@ def build_parser() -> argparse.ArgumentParser:
 
     model_grp = parser.add_argument_group("model_params")
     model_grp.add_argument("--model_name", default=models.__all__[0], type=str, help="classname of the model to use.",
-                           choices=models.__all__[:3])
+                           choices=models.__all__[:4])
     model_grp.add_argument("--data_pipeline", default="ImageFilesDataPipeline", help="classname of the data pipeline to use.",
                            choices=data_pipeline.__all__)
     model_grp.add_argument("--net_input_size", default=256, type=int, help="size of the network's lowres image input.")
@@ -261,6 +268,7 @@ USM_KEYS = ("train/usm_blur_sigma", "train/usm_sharpen")
 
 
 PYRAMID_FLAGS = "--train_guide --guide_batch_stats"
+CURVES_MODELS = ("HDRNetCurves", "HDRNetGaussianPyr")   # their guides have no batch norm
 
 
 def refuse_untrainable(params, train_guide=False, guide_batch_stats=False, coefficient_batch_stats=False) -> None:
@@ -269,14 +277,14 @@ def refuse_untrainable(params, train_guide=False, guide_batch_stats=False, coeff
     norm without ``coefficient_batch_stats`` and (with ``train_guide``) the pointwise-NN guide without
     ``guide_batch_stats``.  Asks the models themselves, on the CPU, with a stand-in variable that
     requires grad (they refuse before any device work).  ValueError for ``guide_batch_stats`` on
-    ``HDRNetCurves``, whose guide has no batch norm, for ``coefficient_batch_stats`` without
+    ``HDRNetCurves`` and ``HDRNetGaussianPyr``, whose guides have no batch norm, for ``coefficient_batch_stats`` without
     ``batch_norm``, and for ``coefficient_batch_stats`` on the models with a batch-normed guide without
     ``guide_batch_stats`` (the reference runs every batch norm of the model in training mode)."""
     S = int(params["net_input_size"])
     if coefficient_batch_stats and not params["batch_norm"]:
         raise ValueError("--coefficient_batch_stats runs the coefficient network's batch norm in training mode; "
                          "it needs --batch_norm")
-    if coefficient_batch_stats and params["model_name"] != "HDRNetCurves" and not guide_batch_stats:
+    if coefficient_batch_stats and params["model_name"] not in CURVES_MODELS and not guide_batch_stats:
         raise ValueError(f"--coefficient_batch_stats with {params['model_name']} needs --guide_batch_stats: the "
                          "reference runs every batch norm of the model, the guide's included, in training mode")
     if params["model_name"] == "HDRNetGaussianPyrNN" and not (train_guide and guide_batch_stats):
@@ -298,6 +306,9 @@ def refuse_untrainable(params, train_guide=False, guide_batch_stats=False, coeff
     if guide_batch_stats and params["model_name"] == "HDRNetCurves":
         raise ValueError("--guide_batch_stats runs the pointwise-NN guide's batch norm in training mode; "
                          "HDRNetCurves' guide has no batch norm")
+    if guide_batch_stats and params["model_name"] == "HDRNetGaussianPyr":
+        raise ValueError("--guide_batch_stats runs the pointwise-NN guide's batch norm in training mode; "
+                         "HDRNetGaussianPyr's guides are curves, with no batch norm")
     if train_guide and not guide_batch_stats and params["model_name"] == "HDRNetPointwiseNNGuide":
         probe = {GUIDE + "conv2/weights": torch.zeros(1, requires_grad=True)}
         try:

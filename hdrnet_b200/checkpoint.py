@@ -473,6 +473,9 @@ def guide_bins(weights: dict, model_name: str) -> dict:
             out[f"guide_level{lvl}_conv1.bin"] = c1
             out[f"guide_level{lvl}_conv2.bin"] = c2
         return out
+    if model_name == "HDRNetGaussianPyr":
+        raise ValueError("HDRNetGaussianPyr has no guide dumps: freeze_graph.py has no layout for its three curves "
+                         "guides (checkpoint.freeze_model writes its frozen model file)")
     raise ValueError(f"unknown model {model_name}")
 
 
@@ -646,6 +649,10 @@ def import_checkpoint(checkpoint_dir: str, verify: bool = False, legacy: bool = 
 FROZEN_MAGIC = b"HDRNETFZ"
 FROZEN_VERSION = 1
 FROZEN_KINDS = ("HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN")   # kind = index
+# Every model a frozen file holds, kind = index (HDRNET_MODEL_*): FROZEN_KINDS, the first three kinds,
+# then HDRNetGaussianPyr (3).  FROZEN_KINDS keeps naming the first three for callers that describe only those.
+FROZEN_MODEL_NAMES = FROZEN_KINDS + ("HDRNetGaussianPyr",)
+_CURVES_GUIDE_MODELS = ("HDRNetCurves", "HDRNetGaussianPyr")   # guide width 16: the curves' knots
 _FROZEN_HEADER = struct.Struct("<8sII5iI")
 
 
@@ -653,14 +660,14 @@ def frozen_arrays(weights: dict, params: dict) -> list:
     """The arrays of the frozen file, in its order, as float32 numpy: each coefficient-network layer's
     weights and bias (an empty array for a layer without one) as ``models._Prepared`` builds them --
     batch norm folded by ``models._fold`` -- then the guide: the curves guide's ccm, ccm_bias, shifts,
-    slopes, mix and [mix_bias], or the folded w1, b1, w2 and [b2] of each pointwise-NN guide (one per
-    pyramid level)."""
+    slopes, mix and [mix_bias] of each curves guide, or the folded w1, b1, w2 and [b2] of each
+    pointwise-NN guide (one guide per pyramid level)."""
     import torch
 
     from . import models
     name = params.get("model_name", "HDRNetCurves")
-    if name not in FROZEN_KINDS:
-        raise ValueError(f"model_name {name!r} is not one of {FROZEN_KINDS}")
+    if name not in FROZEN_MODEL_NAMES:
+        raise ValueError(f"model_name {name!r} is not one of {FROZEN_MODEL_NAMES}")
     prep = models._Prepared(weights, params, torch.device("cpu"), getattr(models, name)._nn_guide)
     out = []
     for scope, _, _ in models._coefficient_specs(params):
@@ -689,10 +696,10 @@ def freeze_model(weights: dict, params: dict, path: str) -> str:
     ``hdrnet_b200.frozen.FrozenModel``, and the ``hdrnet_run`` program) load.  Returns `path`."""
     arrays = frozen_arrays(weights, params)
     name = params.get("model_name", "HDRNetCurves")
-    width = 16 if name == "HDRNetCurves" else int(arrays[-4].shape[1])
+    width = 16 if name in _CURVES_GUIDE_MODELS else int(arrays[-4].shape[1])
     hyper = (int(params["net_input_size"]), int(params["spatial_bin"]), int(params["luma_bins"]),
              int(params["channel_multiplier"]), width)
-    data = _frozen_bytes(FROZEN_KINDS.index(name), hyper, arrays)
+    data = _frozen_bytes(FROZEN_MODEL_NAMES.index(name), hyper, arrays)
     with open(path, "wb") as f:
         f.write(data)
     return path
@@ -711,7 +718,7 @@ def read_frozen_model(path: str) -> dict:
         raise ValueError(f"{path}: frozen model format version {version}, this reader knows {FROZEN_VERSION}")
     if crc32c(data[:-4]) != struct.unpack_from("<I", data, len(data) - 4)[0]:
         raise ValueError(f"{path}: CRC-32C mismatch")
-    if kind >= len(FROZEN_KINDS):
+    if kind >= len(FROZEN_MODEL_NAMES):
         raise ValueError(f"{path}: unknown model kind {kind}")
     arrays, off = [], _FROZEN_HEADER.size
     end = len(data) - 4
@@ -730,5 +737,5 @@ def read_frozen_model(path: str) -> dict:
         off += 4 * count
     if off != end:
         raise ValueError(f"{path}: {end - off} bytes after the last array")
-    return dict(model_name=FROZEN_KINDS[kind], net_input_size=S, spatial_bin=sb, luma_bins=gd,
+    return dict(model_name=FROZEN_MODEL_NAMES[kind], net_input_size=S, spatial_bin=sb, luma_bins=gd,
                 channel_multiplier=cm, guide_width=width, arrays=arrays)

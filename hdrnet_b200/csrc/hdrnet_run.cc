@@ -113,6 +113,7 @@ const char* kind_name(int kind) {
     case HDRNET_MODEL_CURVES: return "HDRNetCurves";
     case HDRNET_MODEL_POINTWISE_NN: return "HDRNetPointwiseNNGuide";
     case HDRNET_MODEL_GAUSSIAN_PYR_NN: return "HDRNetGaussianPyrNN";
+    case HDRNET_MODEL_GAUSSIAN_PYR: return "HDRNetGaussianPyr";
     default: return "unknown";
   }
 }

@@ -17,7 +17,8 @@
 //   fc2, fc3, local conv1, conv2, prediction conv1) as its weights (conv HWIO, fc [in][out]) and
 //   its bias ([cout]; dims [0] for local conv2, which has none); then the guide: ccm [3,3],
 //   ccm_bias [3], shifts [3,16], slopes [3,16], mix [3], mix_bias [1] for the curves guide, or
-//   w1 [3,F], b1 [F], w2 [F], b2 [1] for the pointwise-NN guide, once per pyramid level (0, 1, 2).
+//   w1 [3,F], b1 [F], w2 [F], b2 [1] for the pointwise-NN guide, once per pyramid level (0, 1, 2)
+//   for the two pyramid kinds.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -73,7 +74,9 @@ struct LayerSpec { int k, cin, cout, stride, relu, bias; };
 
 struct Hyper { int kind, S, sb, gd, cm, feats; };
 
-int n_out_of(int kind) { return kind == HDRNET_MODEL_GAUSSIAN_PYR_NN ? 9 : 3; }
+bool is_pyramid(int kind) { return kind == HDRNET_MODEL_GAUSSIAN_PYR_NN || kind == HDRNET_MODEL_GAUSSIAN_PYR; }
+bool has_curves_guide(int kind) { return kind == HDRNET_MODEL_CURVES || kind == HDRNET_MODEL_GAUSSIAN_PYR; }
+int n_out_of(int kind) { return is_pyramid(kind) ? 9 : 3; }
 
 // models._coefficient_specs and init_weights' shapes; false when the hyperparameters are invalid.
 bool layer_specs(const Hyper& h, std::vector<LayerSpec>* out, int* n_ds) {
@@ -117,19 +120,19 @@ void expected_shapes(const Hyper& h, const std::vector<LayerSpec>& L, std::vecto
     else s->push_back({uint32_t(l.cin), uint32_t(l.cout)});
     s->push_back({uint32_t(l.bias ? l.cout : 0)});
   }
-  if (h.kind == HDRNET_MODEL_CURVES) {
-    for (const auto& d : std::vector<std::vector<uint32_t>>{{3, 3}, {3}, {3, 16}, {3, 16}, {3}, {1}}) s->push_back(d);
-  } else {
-    const int levels = h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN ? 3 : 1;
-    const uint32_t F = static_cast<uint32_t>(h.feats);
-    for (int l = 0; l < levels; ++l)
-      for (const auto& d : std::vector<std::vector<uint32_t>>{{3, F}, {F}, {F}, {1}}) s->push_back(d);
-  }
+  const int levels = is_pyramid(h.kind) ? 3 : 1;
+  const uint32_t F = static_cast<uint32_t>(h.feats);
+  const std::vector<std::vector<uint32_t>> guide =
+      has_curves_guide(h.kind) ? std::vector<std::vector<uint32_t>>{{3, 3}, {3}, {3, 16}, {3, 16}, {3}, {1}}
+                               : std::vector<std::vector<uint32_t>>{{3, F}, {F}, {F}, {1}};
+  for (int l = 0; l < levels; ++l)
+    for (const auto& d : guide) s->push_back(d);
 }
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct NNGuideHost { float w1[3 * 32], b1[32], w2[32], b2; int feats; };
+struct CurvesGuideHost { float ccm[9], ccm_bias[3], shifts[48], slopes[48], mix[3], mix_bias; };
 
 }  // namespace
 
@@ -143,8 +146,8 @@ struct hdrnet_model {
   const float* w[kMaxLayers];
   const float* b[kMaxLayers];             // NULL: no bias
   const float* packed[kMaxLayers];        // tensor-core packed conv weights, or NULL
-  // guides: host arrays (the kernels take them in their argument block)
-  float ccm[9], ccm_bias[3], shifts[48], slopes[48], mix[3], mix_bias;
+  // guides, one per pyramid level: host arrays (the kernels take them in their argument block)
+  CurvesGuideHost curves[3];
   NNGuideHost nn[3];
 };
 
@@ -171,9 +174,9 @@ int parse_blob(const unsigned char* p, size_t bytes, Hyper* h, std::vector<Layer
   h->cm = static_cast<int>(rd_u32(p + 28));
   h->feats = static_cast<int>(rd_u32(p + 32));
   if (h->kind != HDRNET_MODEL_CURVES && h->kind != HDRNET_MODEL_POINTWISE_NN &&
-      h->kind != HDRNET_MODEL_GAUSSIAN_PYR_NN)
+      h->kind != HDRNET_MODEL_GAUSSIAN_PYR_NN && h->kind != HDRNET_MODEL_GAUSSIAN_PYR)
     return HDRNET_E_BAD_MODEL;
-  if (h->kind == HDRNET_MODEL_CURVES ? h->feats != 16 : (h->feats < 1 || h->feats > 32)) return HDRNET_E_BAD_MODEL;
+  if (has_curves_guide(h->kind) ? h->feats != 16 : (h->feats < 1 || h->feats > 32)) return HDRNET_E_BAD_MODEL;
   if (!layer_specs(*h, L, n_ds)) return HDRNET_E_BAD_MODEL;
   std::vector<std::vector<uint32_t>> shapes;
   expected_shapes(*h, *L, &shapes);
@@ -244,7 +247,7 @@ void layout(const hdrnet_model* m, int B, int H, int W, int in_fmt, int out_fmt,
   l->grid = c.take(static_cast<size_t>(B) * h.sb * h.sb * h.gd * n_out_of(h.kind) * 4 * f);
   l->acts_bytes = hdrnet_coefficients_scratch_bytes(B, h.S, h.sb, h.gd, h.cm, n_out_of(h.kind), 4);
   l->acts = c.take(l->acts_bytes);
-  if (h.kind != HDRNET_MODEL_GAUSSIAN_PYR_NN) {
+  if (!is_pyramid(h.kind)) {
     if (in_fmt == HDRNET_PX_F32 && out_fmt == HDRNET_PX_F32) l->gmap = c.take(npx * f);
     if (texture_form_runs(B, H, W, h.gd, h.sb)) {
       l->slab_bytes = hdrnet_slice_apply_workspace_bytes(B, H, h.sb, h.gd);
@@ -279,7 +282,7 @@ void layout_ragged(const hdrnet_model* m, const hdrnet_image_desc* images, int B
   l->grid = c.take(static_cast<size_t>(B) * h.sb * h.sb * h.gd * n_out_of(h.kind) * 4 * f);
   l->acts_bytes = hdrnet_coefficients_scratch_bytes(B, h.S, h.sb, h.gd, h.cm, n_out_of(h.kind), 4);
   l->acts = c.take(l->acts_bytes);
-  if (h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN) {
+  if (is_pyramid(h.kind)) {
     size_t lp[3] = {0, 0, 0};
     for (int i = 0; i < B; ++i) {
       const int H = images[i].H, W = images[i].W;
@@ -374,10 +377,11 @@ int coefficients(const hdrnet_model* m, const float* lowres, float* grid, float*
 int slice_apply(const hdrnet_model* m, int level, const float* grid, const void* in, int in_fmt, void* out,
                 int out_fmt, float* gmap, int B, int H, int W, float* slab, size_t slab_bytes, cudaStream_t st) {
   const Hyper& h = m->h;
-  if (h.kind == HDRNET_MODEL_CURVES)
-    return hdrnet_slice_apply_curves_px_ws(grid, in, in_fmt, out, out_fmt, gmap, B, H, W, h.sb, h.sb, h.gd,
-                                           m->ccm, m->ccm_bias, m->shifts, m->slopes, m->mix, m->mix_bias,
-                                           slab, slab_bytes, st);
+  if (has_curves_guide(h.kind)) {
+    const CurvesGuideHost& g = m->curves[level];
+    return hdrnet_slice_apply_curves_px_ws(grid, in, in_fmt, out, out_fmt, gmap, B, H, W, h.sb, h.sb, h.gd, g.ccm,
+                                           g.ccm_bias, g.shifts, g.slopes, g.mix, g.mix_bias, slab, slab_bytes, st);
+  }
   const NNGuideHost& g = m->nn[level];
   return hdrnet_slice_apply_nn_px_ws(grid, in, in_fmt, out, out_fmt, gmap, B, H, W, h.sb, h.sb, h.gd, g.w1, g.b1,
                                      g.w2, g.b2, g.feats, slab, slab_bytes, st);
@@ -396,7 +400,7 @@ split_level_rows_kernel(const float* __restrict__ coeffs, float* __restrict__ c0
   }
 }
 
-// HDRNetGaussianPyrNN.inference_image after the coefficients: the float image, its two smaller
+// HDRNetGaussianPyrNN.inference_image (and HDRNetGaussianPyr's) after the coefficients: the float image, its two smaller
 // levels, one fused slice-apply per level with its three coefficient rows `coef` (level il's rows
 // [B, sb, sb, gd, 12]), coarse-to-fine upsample-and-add.  `l` holds the intermediates for B x H x W.
 int pyramid_fullres(const hdrnet_model* m, const Layout& l, const float* const coef[3], const void* image,
@@ -493,15 +497,18 @@ int hdrnet_model_create(const void* blob, size_t bytes, hdrnet_model** out) {
   }
   // guides: host copies
   size_t a = 2 * n_layers;
-  if (h.kind == HDRNET_MODEL_CURVES) {
-    read_floats(arrays[a], m->ccm, 9);
-    read_floats(arrays[a + 1], m->ccm_bias, 3);
-    read_floats(arrays[a + 2], m->shifts, 48);
-    read_floats(arrays[a + 3], m->slopes, 48);
-    read_floats(arrays[a + 4], m->mix, 3);
-    read_floats(arrays[a + 5], &m->mix_bias, 1);
+  const int levels = is_pyramid(h.kind) ? 3 : 1;
+  if (has_curves_guide(h.kind)) {
+    for (int l = 0; l < levels; ++l, a += 6) {
+      CurvesGuideHost& g = m->curves[l];
+      read_floats(arrays[a], g.ccm, 9);
+      read_floats(arrays[a + 1], g.ccm_bias, 3);
+      read_floats(arrays[a + 2], g.shifts, 48);
+      read_floats(arrays[a + 3], g.slopes, 48);
+      read_floats(arrays[a + 4], g.mix, 3);
+      read_floats(arrays[a + 5], &g.mix_bias, 1);
+    }
   } else {
-    const int levels = h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN ? 3 : 1;
     for (int l = 0; l < levels; ++l, a += 4) {
       NNGuideHost& g = m->nn[l];
       g.feats = h.feats;
@@ -562,7 +569,7 @@ int hdrnet_model_run_px(const hdrnet_model* m, const void* image, int in_fmt, co
   if (cudaGetDevice(&dev) != cudaSuccess || dev != m->device) return HDRNET_E_BAD_CONTEXT;
   if (!valid_fmt(in_fmt) || !valid_fmt(out_fmt) || (lowres_image && !valid_fmt(lowres_fmt)))
     return HDRNET_E_UNSUPPORTED;
-  const bool pyr = m->h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN;
+  const bool pyr = is_pyramid(m->h.kind);
   if (B < 0 || H < 0 || W < 0 || (lowres_image && (SH < 1 || SW < 1))) return HDRNET_E_BAD_SHAPE;
   const long long npx = static_cast<long long>(B) * H * W;
   if (npx == 0) return HDRNET_OK;
@@ -591,7 +598,7 @@ int hdrnet_model_run_px(const hdrnet_model* m, const void* image, int in_fmt, co
     return slice_apply(m, 0, l.grid, image, in_fmt, out, out_fmt, gmap, B, H, W, l.slab, l.slab_bytes, st);
   }
 
-  // HDRNetGaussianPyrNN.inference_image: the float image, its two smaller levels, one fused
+  // the pyramids' inference_image: the float image, its two smaller levels, one fused
   // slice-apply per level with its three coefficient rows, coarse-to-fine upsample-and-add
   const long long cells = static_cast<long long>(B) * h.sb * h.sb * h.gd;
   split_level_rows_kernel<<<static_cast<unsigned>(std::min<long long>((cells * 36 + 255) / 256, 132LL * 32)), 256, 0,
@@ -619,7 +626,7 @@ int hdrnet_model_run_ragged_px(const hdrnet_model* m, const hdrnet_image_desc* i
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess || dev != m->device) return HDRNET_E_BAD_CONTEXT;
   if (!valid_fmt(in_fmt) || !valid_fmt(out_fmt) || (lowres && !valid_fmt(lowres_fmt))) return HDRNET_E_UNSUPPORTED;
-  const bool pyr = m->h.kind == HDRNET_MODEL_GAUSSIAN_PYR_NN;
+  const bool pyr = is_pyramid(m->h.kind);
   int rc = hdrnet_b200::validate_ragged(images, B, in_fmt, out_fmt, true, pyr ? 4 : 1);
   if (rc != HDRNET_OK || B == 0) return rc;
   if (lowres && (rc = hdrnet_b200::validate_ragged(lowres, B, lowres_fmt, out_fmt, false, 1)) != HDRNET_OK) return rc;
@@ -635,10 +642,11 @@ int hdrnet_model_run_ragged_px(const hdrnet_model* m, const hdrnet_image_desc* i
   if (!rc) rc = coefficients(m, l.lowres, l.grid, l.acts, l.acts_bytes, B, st);
   if (rc) return rc;
   if (!pyr) {
-    if (h.kind == HDRNET_MODEL_CURVES)
-      return hdrnet_slice_apply_curves_ragged_px_ws(l.grid, images, B, in_fmt, out_fmt, h.sb, h.sb, h.gd, m->ccm,
-                                                    m->ccm_bias, m->shifts, m->slopes, m->mix, m->mix_bias, nullptr,
-                                                    0, st);
+    if (h.kind == HDRNET_MODEL_CURVES) {
+      const CurvesGuideHost& g = m->curves[0];
+      return hdrnet_slice_apply_curves_ragged_px_ws(l.grid, images, B, in_fmt, out_fmt, h.sb, h.sb, h.gd, g.ccm,
+                                                    g.ccm_bias, g.shifts, g.slopes, g.mix, g.mix_bias, nullptr, 0, st);
+    }
     const NNGuideHost& g = m->nn[0];
     return hdrnet_slice_apply_nn_ragged_px_ws(l.grid, images, B, in_fmt, out_fmt, h.sb, h.sb, h.gd, g.w1, g.b1, g.w2,
                                               g.b2, g.feats, nullptr, 0, st);

@@ -1,10 +1,10 @@
 """A frozen model (``checkpoint.freeze_model``) run through the whole-model C-ABI
 (``hdrnet_model_*``, include/hdrnet_b200.h): the object a C or C++ caller would hold, owned from
 Python.  Its results are bit for bit those of ``models.*.inference_image`` on the same weights, with one
-exception: the pyramid from uint8 / uint16 pixels converts the image with the bit-exact img_as_float,
-where ``inference_image`` divides through torch (``models.image_to_float``, DESIGN.md row f-11); its
-results are bit for bit ``HDRNetGaussianPyrNN.inference`` on the host's img_as_float, then
-``quantize_u8`` / ``quantize_u16``.
+exception: the pyramids from uint8 / uint16 pixels convert the image with the bit-exact img_as_float,
+where ``inference_image`` divides through torch (``models.image_to_float``, DESIGN.md row f-11); their
+results are bit for bit ``HDRNetGaussianPyrNN.inference`` (or ``HDRNetGaussianPyr.inference``) on the
+host's img_as_float, then ``quantize_u8`` / ``quantize_u16``.
 
     model = FrozenModel("frozen_model.hdrnet")            # weights uploaded to the current device
     out = model(image_u8)                                  # [B,H,W,3] uint8 -> uint8, current stream
@@ -25,7 +25,7 @@ import ctypes
 import torch
 
 from . import _lib
-from .checkpoint import FROZEN_KINDS
+from .checkpoint import FROZEN_MODEL_NAMES
 from .models import OUT_DTYPES, _PX_FMT, _check_image, _check_images, _check_out_dtype
 
 
@@ -50,7 +50,7 @@ class FrozenModel:
         _lib.check(lib.hdrnet_model_info(handle, *[ctypes.byref(v) for v in vals]), "model info")
         kind, self.net_input_size, self.spatial_bin, self.luma_bins, self.channel_multiplier, self.guide_width = (
             v.value for v in vals)
-        self.model_name = FROZEN_KINDS[kind]
+        self.model_name = FROZEN_MODEL_NAMES[kind]
 
     @property
     def handle(self) -> ctypes.c_void_p:

@@ -39,7 +39,9 @@ pyramid level (``inference/guide/level_{0,1,2}``): ``inference(..., is_training=
 level with its own batch statistics and moves that level's moving averages, and differentiates the
 coefficient network and, with ``params['guide_grad']``, every level's guide and ``fullres_input``,
 through ``_ResizeFn``, whose backward is the VJP of the align-corners resize (``csrc/resize.cu``); its
-inference form is not differentiated.  Batch-norm layers of the coefficient network are not
+inference form is not differentiated.  ``HDRNetGaussianPyr`` is that pyramid with a curves guide per
+level (DESIGN.md row f-17); with ``params['guide_grad']`` each level's curves variables and
+``fullres_input`` are differentiated through ``_CurvesGuideFn`` and ``_ResizeFn``.  Batch-norm layers of the coefficient network are not
 differentiated in their folded inference form: asking for their gradient raises
 ``NotImplementedError``.  With ``params['coefficient_batch_stats']`` (and ``batch_norm``),
 ``inference(..., is_training=True)`` runs them in training mode (``_coefficients_training``, the kernels
@@ -65,8 +67,8 @@ from . import _lib, layers, parallel
 from .hdrnet_ops import _slice_apply_workspace, _workspace
 from .layers import bilateral_slice_apply
 
-__all__ = ["HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN", "set_weights", "load_weights",
-           "init_weights", "DEFAULT_PARAMS"]
+__all__ = ["HDRNetCurves", "HDRNetPointwiseNNGuide", "HDRNetGaussianPyrNN", "HDRNetGaussianPyr", "set_weights",
+           "load_weights", "init_weights", "DEFAULT_PARAMS"]
 
 BN_EPS = 1e-3   # tf.contrib.layers.batch_norm default epsilon (hdrnet/layers.py:47-54)
 BN_DECAY = 0.999  # ... and its moving-average decay
@@ -111,7 +113,8 @@ def init_weights(params, seed: int = 0, model_name: str | None = None) -> dict:
     """Fresh variables with the reference's initialisers: variance-scaling (fan-in, factor 2,
     truncated normal) for conv/fc weights and zero biases (hdrnet/layers.py:22-23), identity
     ccm / linspace shifts / unit first slope / 1/3 mixing for the curves guide
-    (hdrnet/models.py:150-186).  Used for synthetic-weight benchmarks."""
+    (hdrnet/models.py:150-186), one curves guide per level for HDRNetGaussianPyr, each ccm with its own
+    jitter.  Used for synthetic-weight benchmarks."""
     rng = np.random.RandomState(seed)
     gd, cm = params["luma_bins"], params["channel_multiplier"]
     bn = bool(params["batch_norm"])
@@ -156,24 +159,31 @@ def init_weights(params, seed: int = 0, model_name: str | None = None) -> dict:
     fc(f"{p}/global/fc3", 16 * cm * gd, c8)
     conv(f"{p}/local/conv1", 3, cin, c8, use_bn=bn)
     conv(f"{p}/local/conv2", 3, c8, c8, use_bias=False)
-    n_out = 9 if model_name == "HDRNetGaussianPyrNN" else 3
+    n_out = 9 if model_name in ("HDRNetGaussianPyrNN", "HDRNetGaussianPyr") else 3
     conv(f"{p}/prediction/conv1", 1, c8, gd * n_out * 4)
     g = "inference/guide"
+
+    def curves(scope):   # models.py:152 draws the ccm's jitter once per call
+        w[scope + "/ccm"] = (np.identity(3) + rng.randn(1) * 1e-4).astype(np.float32)
+        w[scope + "/ccm_bias"] = np.zeros(3, np.float32)
+        w[scope + "/shifts"] = np.tile(np.linspace(0, 1, 16, endpoint=False, dtype=np.float32)
+                                       [None, None, None, :], (1, 1, 3, 1))
+        slopes = np.zeros((1, 1, 1, 3, 16), np.float32)
+        slopes[..., 0] = 1.0
+        w[scope + "/slopes"] = slopes
+        w[scope + "/channel_mixing/weights"] = np.full((1, 1, 3, 1), 1.0 / 3.0, np.float32)
+        w[scope + "/channel_mixing/biases"] = np.zeros(1, np.float32)
+
     if model_name == "HDRNetGaussianPyrNN":
         nf = params["guide_complexity"]
         for lvl in range(3):
             conv(f"{g}/level_{lvl}/conv1", 1, 3, nf, use_bn=True)
             conv(f"{g}/level_{lvl}/conv2", 1, nf, 1)
+    elif model_name == "HDRNetGaussianPyr":
+        for lvl in range(3):
+            curves(f"{g}/level_{lvl}")
     elif model_name == "HDRNetCurves":
-        w[g + "/ccm"] = (np.identity(3) + rng.randn(1) * 1e-4).astype(np.float32)
-        w[g + "/ccm_bias"] = np.zeros(3, np.float32)
-        w[g + "/shifts"] = np.tile(np.linspace(0, 1, 16, endpoint=False, dtype=np.float32)
-                                   [None, None, None, :], (1, 1, 3, 1))
-        slopes = np.zeros((1, 1, 1, 3, 16), np.float32)
-        slopes[..., 0] = 1.0
-        w[g + "/slopes"] = slopes
-        w[g + "/channel_mixing/weights"] = np.full((1, 1, 3, 1), 1.0 / 3.0, np.float32)
-        w[g + "/channel_mixing/biases"] = np.zeros(1, np.float32)
+        curves(g)
     else:
         nf = params["guide_complexity"]
         conv(g + "/conv1", 1, 3, nf, use_bn=True)
@@ -285,8 +295,8 @@ class _CurvesGuide:
         self.args = (*[_hp(a) for a in arrays], self.mix_bias)
 
     @classmethod
-    def from_weights(cls, wts):
-        return cls(*[wts["inference/guide/" + n] for n in _CURVES_VARS])
+    def from_weights(cls, wts, scope="inference/guide"):
+        return cls(*[wts[f"{scope}/{n}"] for n in _CURVES_VARS])
 
     def run(self, x: torch.Tensor) -> torch.Tensor:
         """The standalone guide kernel over x [B, H, W, 3] (float32, contiguous) -> [B, H, W]."""
@@ -331,7 +341,9 @@ class _NNGuide:
 
 class _Prepared:
     """Device copies of the coefficient-network weights + the guide's host parameters: `guides`, one
-    _CurvesGuide or _NNGuide, or one _NNGuide per level of the pyramid model."""
+    _CurvesGuide or _NNGuide, or one per level of a pyramid model.  `nn_guide` is the model's
+    _nn_guide: False (curves), True (pointwise NN), "pyramid" (an NN guide per level) or
+    "curves_pyramid" (a curves guide per level)."""
 
     def __init__(self, wts, params, device, nn_guide):
         self.device = device
@@ -345,6 +357,8 @@ class _Prepared:
         g = "inference/guide"
         if nn_guide == "pyramid":     # HDRNetGaussianPyrNN: one pointwise NN per level
             self.guides = [_NNGuide.folded(wts, f"{g}/level_{lvl}") for lvl in range(3)]
+        elif nn_guide == "curves_pyramid":     # HDRNetGaussianPyr: one curves guide per level
+            self.guides = [_CurvesGuide.from_weights(wts, f"{g}/level_{lvl}") for lvl in range(3)]
         elif nn_guide:
             self.guides = [_NNGuide.folded(wts, g)]
         else:
@@ -1006,13 +1020,14 @@ def _trainable_keys(wts, prefix: str):
 
 
 def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=None, nn_guide=False,
-                      is_training=False, bn_training=False) -> None:
+                      is_training=False, bn_training=False, curves_model="HDRNetCurves") -> None:
     """NotImplementedError for every gradient this package does not compute (checked before any
     device work).  `what`: refuse the whole model's gradient (HDRNetGaussianPyrNN's inference form).
     The curves guide's variables and fullres_input are differentiated only with params['guide_grad'], the
     pointwise-NN guide's only with params['guide_grad'] and `is_training` (training-mode batch norm).
     `bn_training`: the coefficient network's batch-norm layers run in training mode
-    (_coefficient_batch_stats), so their variables may require grad."""
+    (_coefficient_batch_stats), so their variables may require grad.  `curves_model`: the curves-guide
+    model the messages name."""
     if not torch.is_grad_enabled() or wts is None:
         return
     if what is not None:
@@ -1032,7 +1047,7 @@ def _refuse_untrained(wts, params, lowres_input=None, fullres_input=None, what=N
             "requires grad): its conv1 has batch norm, which training runs in training mode with batch "
             "statistics, a different forward; inference(..., is_training=True) runs that forward and "
             "differentiates it")
-    hint = "; params['guide_grad'] computes them for HDRNetCurves"
+    hint = f"; params['guide_grad'] computes them for {curves_model}"
     if guide and not guide_grad:
         raise NotImplementedError(f"gradients for the guide variables are not implemented ({guide[0]} requires "
                                   "grad): the guide is held fixed; set requires_grad=False on its variables"
@@ -1304,16 +1319,17 @@ class HDRNetCurves(object):
         return grid
 
     @classmethod
-    def _guide(cls, input_tensor, params, is_training=False):
+    def _guide(cls, input_tensor, params, is_training=False, scope=GUIDE):
         """models.py:145-190 as a standalone kernel -> [B, H, W].  Differentiable (_CurvesGuideFn)
-        when _guide_grad says so."""
+        when _guide_grad says so.  ``scope``: the guide's variable scope (the pyramid's
+        GUIDE/level_{l})."""
         x = _check_input(input_tensor, "fullres_input")
         wts = _resolve_weights(params)
-        if _guide_grad(wts, params, x, _CURVES_VARS):
+        if _guide_grad(wts, params, x, _CURVES_VARS, scope):
             with torch.cuda.device(x.device):
-                return _CurvesGuideFn.apply(x, *[wts["inference/guide/" + n] for n in _CURVES_VARS])
-        if is_training:    # the coefficient layers are not prepared (folded, packed) for the guide alone
-            return _CurvesGuide.from_weights(wts).run(x)
+                return _CurvesGuideFn.apply(x, *[wts[f"{scope}/{n}"] for n in _CURVES_VARS])
+        if is_training or scope != GUIDE:   # the coefficient layers are not prepared (folded, packed) for the guide alone
+            return _CurvesGuide.from_weights(wts, scope).run(x)
         return _prepare(wts, params, x.device, False).guides[0].run(x)
 
     @classmethod
@@ -1435,15 +1451,13 @@ def _resize_maybe_grad(x, oh, ow, add=None):
     return _resize(x, oh, ow, add)
 
 
-class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
-    """Replace input to the affine model by a pyramid (hdrnet/models.py:213-289): 3-level
-    bilinear (align_corners) pyramid of the full-res image, one pointwise-NN guide per level,
-    one slice-apply per level with its own 3 of the 9 output rows of the coefficient grid,
-    coarse-to-fine upsample-and-add.  The reference file is Python-2 only here
-    (`reversed(zip(...))`, :278); the semantics restated: the COARSEST level uses output rows
-    0..2, the finest rows 6..8."""
-
-    _nn_guide = "pyramid"
+class _GaussianPyramid:
+    """The pyramid of hdrnet/models.py:213-289, shared by HDRNetGaussianPyrNN and HDRNetGaussianPyr,
+    which differ only in the guide each level runs (their _nn_guide and _guide): 3-level bilinear
+    (align_corners) pyramid of the full-res image, one guide per level, one slice-apply per level
+    with its own 3 of the 9 output rows of the coefficient grid, coarse-to-fine upsample-and-add.
+    The reference file is Python-2 only here (`reversed(zip(...))`, :278); the semantics restated:
+    the COARSEST level uses output rows 0..2, the finest rows 6..8."""
 
     @classmethod
     def n_scales(cls):
@@ -1456,6 +1470,81 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
     @classmethod
     def n_in(cls):
         return 3 + 1
+
+    @classmethod
+    def _guide_scopes(cls):
+        return [f"{GUIDE}/level_{il}" for il in range(cls.n_scales())]
+
+    @classmethod
+    def inference_image(cls, image, params, lowres_image=None, out_dtype=torch.uint8):
+        """Same contract as HDRNetCurves.inference_image.  The pyramid needs the float image at
+        three scales, so only the network input is taken straight from the integer pixels; the
+        full-resolution image is converted once on the device.  The float result of the three
+        levels' sum is quantised once, on the device (quantize_u8 / quantize_u16)."""
+        _check_out_dtype(out_dtype)
+        image = _check_image(image, "image")
+        src = image if lowres_image is None else _check_image(lowres_image, "lowres_image")
+        lowres = lowres_from_image(src, int(params["net_input_size"]))
+        out = cls.inference(lowres, image_to_float(image), params, False)
+        if out_dtype == torch.uint8:
+            return quantize_u8(out)
+        return quantize_u16(out) if out_dtype == torch.uint16 else out
+
+    @classmethod
+    def _fullres_images(cls, coeffs, images, params, out_dtype):
+        """The pyramid over a ragged batch: the coefficients of all the images come from one network
+        call; the full-resolution stages (float image, level resizes, three slice-applies, upsample
+        and add) run image by image, as inference_image runs them on one image (there is no ragged
+        form of the resizes)."""
+        outs = []
+        with torch.cuda.device(images[0].device):
+            for i, image in enumerate(images):
+                out = cls._output(cls._multiscale_input(image_to_float(image[None])), None, coeffs[i:i + 1], params)
+                if out_dtype == torch.uint8:
+                    out = quantize_u8(out)
+                elif out_dtype == torch.uint16:
+                    out = quantize_u16(out)
+                outs.append(out[0])
+        return outs
+
+    @classmethod
+    def _multiscale_input(cls, fullres_input):
+        """models.py:249-262: each level is the previous one resized to floor(size / 2);
+        differentiable (_ResizeFn) when fullres_input requires grad."""
+        lvls = [fullres_input]
+        h, w = fullres_input.shape[1:3]
+        for _ in range(cls.n_scales() - 1):
+            h, w = h // 2, w // 2
+            lvls.append(_resize_maybe_grad(lvls[-1], h, w))
+        return lvls
+
+    @classmethod
+    def _output(cls, lvls, guide_lvls, coeffs, params=None):
+        """models.py:274-289, coarse to fine.  With guide_lvls=None (the fast path) each level's
+        guide is computed inside its slice-apply kernel; given the guides, hdrnet_ops' slice-apply
+        runs on them, and the upsample-and-add is differentiable (_ResizeFn) where grad is on."""
+        prep = _prepare(_resolve_weights(params), params, lvls[0].device, cls._nn_guide) \
+            if guide_lvls is None else None
+        B, gh, gw, gd = coeffs.shape[:4]
+        current = None
+        for il in range(cls.n_scales()):
+            src = cls.n_scales() - 1 - il                       # reversed(zip(lvls, guides))
+            lvl = lvls[src]
+            c = coeffs[:, :, :, :, il * 3:(il + 1) * 3, :].contiguous().reshape(B, gh, gw, gd, 12)
+            _, H, W, _ = lvl.shape
+            if guide_lvls is not None:
+                out_lvl = bilateral_slice_apply(c, guide_lvls[src], lvl, has_offset=True)
+            else:
+                out_lvl = _slice_apply_fused(c, lvl, prep.guides[src], torch.float32, False, False)[0]
+            current = out_lvl if il == 0 else _resize_maybe_grad(current, H, W, add=out_lvl)
+        return current
+
+
+class HDRNetGaussianPyrNN(_GaussianPyramid, HDRNetPointwiseNNGuide):
+    """Replace input to the affine model by a pyramid (hdrnet/models.py:213-289): the pyramid of
+    _GaussianPyramid with one pointwise-NN guide per level."""
+
+    _nn_guide = "pyramid"
 
     @classmethod
     def inference(cls, lowres_input, fullres_input, params, is_training=False):
@@ -1506,53 +1595,6 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
             return cls._output(multiscale, guides, coeffs, params)
 
     @classmethod
-    def _guide_scopes(cls):
-        return [f"{GUIDE}/level_{il}" for il in range(cls.n_scales())]
-
-    @classmethod
-    def inference_image(cls, image, params, lowres_image=None, out_dtype=torch.uint8):
-        """Same contract as HDRNetCurves.inference_image.  The pyramid needs the float image at
-        three scales, so only the network input is taken straight from the integer pixels; the
-        full-resolution image is converted once on the device.  The float result of the three
-        levels' sum is quantised once, on the device (quantize_u8 / quantize_u16)."""
-        _check_out_dtype(out_dtype)
-        image = _check_image(image, "image")
-        src = image if lowres_image is None else _check_image(lowres_image, "lowres_image")
-        lowres = lowres_from_image(src, int(params["net_input_size"]))
-        out = cls.inference(lowres, image_to_float(image), params, False)
-        if out_dtype == torch.uint8:
-            return quantize_u8(out)
-        return quantize_u16(out) if out_dtype == torch.uint16 else out
-
-    @classmethod
-    def _fullres_images(cls, coeffs, images, params, out_dtype):
-        """The pyramid over a ragged batch: the coefficients of all the images come from one network
-        call; the full-resolution stages (float image, level resizes, three slice-applies, upsample
-        and add) run image by image, as inference_image runs them on one image (there is no ragged
-        form of the resizes)."""
-        outs = []
-        with torch.cuda.device(images[0].device):
-            for i, image in enumerate(images):
-                out = cls._output(cls._multiscale_input(image_to_float(image[None])), None, coeffs[i:i + 1], params)
-                if out_dtype == torch.uint8:
-                    out = quantize_u8(out)
-                elif out_dtype == torch.uint16:
-                    out = quantize_u16(out)
-                outs.append(out[0])
-        return outs
-
-    @classmethod
-    def _multiscale_input(cls, fullres_input):
-        """models.py:249-262: each level is the previous one resized to floor(size / 2);
-        differentiable (_ResizeFn) when fullres_input requires grad."""
-        lvls = [fullres_input]
-        h, w = fullres_input.shape[1:3]
-        for _ in range(cls.n_scales() - 1):
-            h, w = h // 2, w // 2
-            lvls.append(_resize_maybe_grad(lvls[-1], h, w))
-        return lvls
-
-    @classmethod
     def _guide(cls, multiscale, params, is_training=False):
         """models.py:264-272: HDRNetPointwiseNNGuide._guide per level (scope level_{il}).  In training
         mode each level is normalised with its own batch statistics and updates its own moving
@@ -1563,26 +1605,56 @@ class HDRNetGaussianPyrNN(HDRNetPointwiseNNGuide):
         prep = _prepare(_resolve_weights(params), params, multiscale[0].device, "pyramid")
         return [guide.run(lvl) for lvl, guide in zip(multiscale, prep.guides)]
 
+
+class HDRNetGaussianPyr(_GaussianPyramid, HDRNetCurves):
+    """HDRNetGaussianPyrNN with HDRNetCurves' guide in place of the pointwise NN: the pyramid of
+    _GaussianPyramid with one curves guide per level (``inference/guide/level_{0,1,2}/{ccm, ccm_bias,
+    shifts, slopes, channel_mixing/*}``).  The reference's gpyr recipes name this model
+    (scripts/ll/train_gpyr.sh, scripts/usm/train_gpyr.sh, scripts/ll_strong/train_gpyrnn*.sh), but its
+    models.py never defines it; this definition is the project's own (DESIGN.md row f-17).  The curves
+    guide has no batch norm, so the inference form is also the training form, as for HDRNetCurves."""
+
+    _nn_guide = "curves_pyramid"
+
     @classmethod
-    def _output(cls, lvls, guide_lvls, coeffs, params=None):
-        """models.py:274-289, coarse to fine.  With guide_lvls=None (the fast path) each level's
-        guide is computed inside its slice-apply kernel; given the guides, hdrnet_ops' slice-apply
-        runs on them, and the upsample-and-add is differentiable (_ResizeFn) where grad is on."""
-        prep = _prepare(_resolve_weights(params), params, lvls[0].device, "pyramid") \
-            if guide_lvls is None else None
-        B, gh, gw, gd = coeffs.shape[:4]
-        current = None
-        for il in range(cls.n_scales()):
-            src = cls.n_scales() - 1 - il                       # reversed(zip(lvls, guides))
-            lvl = lvls[src]
-            c = coeffs[:, :, :, :, il * 3:(il + 1) * 3, :].contiguous().reshape(B, gh, gw, gd, 12)
-            _, H, W, _ = lvl.shape
-            if guide_lvls is not None:
-                out_lvl = bilateral_slice_apply(c, guide_lvls[src], lvl, has_offset=True)
-            else:
-                out_lvl = _slice_apply_fused(c, lvl, prep.guides[src], torch.float32, False, False)[0]
-            current = out_lvl if il == 0 else _resize_maybe_grad(current, H, W, add=out_lvl)
-        return current
+    def inference(cls, lowres_input, fullres_input, params, is_training=False):
+        """lowres_input [B,S,S,3], fullres_input [B,H,W,3] (H, W >= 4) -> [B,H,W,3].  Without
+        gradients each level's curves guide runs inside its slice-apply.  With coefficient-network
+        variables (or lowres_input) requiring grad, the guides come from the standalone kernel and
+        the output from hdrnet_ops' slice-apply and the resize, whose VJPs carry the gradient back to
+        the grid; with params['guide_grad'] each level's curves variables and fullres_input are
+        differentiated too, through _CurvesGuideFn and _ResizeFn.  With params['debug'] the
+        coefficients, the three guide maps and the levels go to ``cls.last_debug``.
+
+        ``is_training=True`` needs params['coefficient_batch_stats'] with params['batch_norm'] (else
+        NotImplementedError): the coefficient network's batch-norm layers then normalise with the
+        batch's statistics, as in HDRNetCurves.inference."""
+        bn_training = _coefficient_batch_stats(params)
+        if is_training and not bn_training:
+            raise NotImplementedError("hdrnet_b200 implements the inference path only")
+        wts = _weights_or_none(params)
+        _refuse_untrained(wts, params, fullres_input=fullres_input, bn_training=bool(is_training),
+                          curves_model=cls.__name__)
+        fullres_input = _check_input(fullres_input, "fullres_input")
+        coeffs = cls._coefficients(lowres_input, params, is_training)       # [B,gh,gw,gd,9,4]
+        debug = bool(params.get("debug"))
+        with torch.cuda.device(fullres_input.device):
+            multiscale = cls._multiscale_input(fullres_input)
+            grad = coeffs.requires_grad or any(_guide_grad(wts, params, lvl, _CURVES_VARS, scope)
+                                               for lvl, scope in zip(multiscale, cls._guide_scopes()))
+            guides = cls._guide(multiscale, params) if grad or debug else None
+            out = cls._output(multiscale, guides, coeffs, params)
+        if debug:
+            cls.last_debug = {"bilateral_coefficients": coeffs, "guide": guides,
+                              "multiscale": multiscale, "output": out}
+        return out
+
+    @classmethod
+    def _guide(cls, multiscale, params, is_training=False):
+        """models.py:264-272 with HDRNetCurves' guide: HDRNetCurves._guide per level (scope
+        level_{il}), each differentiable (_CurvesGuideFn) when _guide_grad says so."""
+        return [HDRNetCurves._guide(lvl, params, is_training, scope)
+                for lvl, scope in zip(multiscale, cls._guide_scopes())]
 
 
 del layers  # imported for the side effect of the public surface only

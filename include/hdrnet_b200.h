@@ -648,13 +648,14 @@ HDRNET_API int hdrnet_slice_apply_host_f32(hdrnet_host_ctx* ctx, const float* gr
                                 int gw, int gd, int n_in, int n_out, int has_offset);
 
 /*
- * A whole trained model (HDRNetCurves, HDRNetPointwiseNNGuide or HDRNetGaussianPyrNN) from its frozen
- * model file (hdrnet_b200.checkpoint.freeze_model; the layout is documented in csrc/model.cu and
- * DESIGN.md row f-12): the C counterpart of models.*.inference_image, running the same kernels chosen
- * by the same rules, so its results are bit for bit that path's -- except the pyramid from uint8 /
- * uint16 pixels, whose full-resolution image is converted with the bit-exact img_as_float here where
- * models.image_to_float divides through torch (DESIGN.md row f-11): there the results are bit for bit
- * HDRNetGaussianPyrNN.inference on the host's img_as_float, quantised as inference_image quantises.
+ * A whole trained model (HDRNetCurves, HDRNetPointwiseNNGuide, HDRNetGaussianPyrNN or
+ * HDRNetGaussianPyr) from its frozen model file (hdrnet_b200.checkpoint.freeze_model; the layout is
+ * documented in csrc/model.cu and DESIGN.md row f-12): the C counterpart of models.*.inference_image,
+ * running the same kernels chosen by the same rules, so its results are bit for bit that path's --
+ * except the pyramids from uint8 / uint16 pixels, whose full-resolution image is converted with the
+ * bit-exact img_as_float here where models.image_to_float divides through torch (DESIGN.md row f-11):
+ * there the results are bit for bit the pyramid's inference on the host's img_as_float, quantised as
+ * inference_image quantises.
  *
  * hdrnet_model_create: checks the whole host blob (magic, format version, lengths, every array's
  *   shape against the hyperparameters, CRC-32C) before any CUDA call -- HDRNET_E_BAD_MODEL for any
@@ -686,6 +687,7 @@ HDRNET_API int hdrnet_slice_apply_host_f32(hdrnet_host_ctx* ctx, const float* gr
 #define HDRNET_MODEL_CURVES 0
 #define HDRNET_MODEL_POINTWISE_NN 1
 #define HDRNET_MODEL_GAUSSIAN_PYR_NN 2
+#define HDRNET_MODEL_GAUSSIAN_PYR 3     /* the pyramid with a curves guide per level */
 
 typedef struct hdrnet_model hdrnet_model;
 
